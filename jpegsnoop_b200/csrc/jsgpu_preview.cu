@@ -99,9 +99,12 @@ template <bool FULLCONV, bool HIST>
 __global__ void __launch_bounds__(PV_THREADS) k_preview(DevBatch b, jsgpu_preview pv, jsgpu_colour_stats* st, uint32_t* rowclip)
 {
     __shared__ PvShared sh;
-    const DevImage& im = b.img[blockIdx.y];
-    if (!im.valid) return;
-    if (HIST) { for (uint32_t i = threadIdx.x; i < sizeof(PvShared) / 4; i += PV_THREADS) reinterpret_cast<uint32_t*>(&sh)[i] = 0; __syncthreads(); }
+    // one image per blockIdx.y, strided beyond 65535 images: a CTA that moves on flushes its histograms and ranges first and
+    // starts the next image from zero
+    for (uint32_t ii = blockIdx.y; ii < b.nimg; ii += gridDim.y) {
+    const DevImage& im = b.img[ii];
+    if (!im.valid) continue;
+    if (HIST) { __syncthreads(); for (uint32_t i = threadIdx.x; i < sizeof(PvShared) / 4; i += PV_THREADS) reinterpret_cast<uint32_t*>(&sh)[i] = 0; __syncthreads(); }
     int vmin[12], vmax[12]; long long vsum[12]; uint32_t rgbclip[6];
     #pragma unroll
     for (int k = 0; k < 12; k++) { vmin[k] = 0; vmax[k] = 0; vsum[k] = 0; }     // memset(&m_sHisto, 0) (:3147): the ranges START at 0
@@ -140,7 +143,7 @@ __global__ void __launch_bounds__(PV_THREADS) k_preview(DevBatch b, jsgpu_previe
                 } else pv_fast(p);
                 sum_fy += p.fy;
                 o[q] = pv_extract(pv.mode, p);
-                if (det) st[blockIdx.y].detail_rgb[py - pv.detail_mcu_y * im.mcu_h][px + q - pv.detail_mcu_x * im.mcu_w] = (p.fr << 16) | (p.fg << 8) | p.fb;   // sPixSrc.nFinalR/G/B (:4763)
+                if (det) st[ii].detail_rgb[py - pv.detail_mcu_y * im.mcu_h][px + q - pv.detail_mcu_x * im.mcu_w] = (p.fr << 16) | (p.fg << 8) | p.fb;   // sPixSrc.nFinalR/G/B (:4763)
             }
             drow[px >> 2] = make_uint4(o[0], o[1], o[2], o[3]);
         }
@@ -149,9 +152,9 @@ __global__ void __launch_bounds__(PV_THREADS) k_preview(DevBatch b, jsgpu_previe
             if ((threadIdx.x & 31) == 0 && row_events) atomicAdd(&rowclip[im.row_off + py], row_events);
         }
     }
-    jsgpu_colour_stats* const o = st + blockIdx.y;
+    jsgpu_colour_stats* const o = st + ii;
     for (int d = 16; d; d >>= 1) sum_fy += __shfl_xor_sync(FULL, sum_fy, d);
-    if ((threadIdx.x & 31) == 0 && sum_fy) atomicAdd(&b.sum_y[blockIdx.y], sum_fy);
+    if ((threadIdx.x & 31) == 0 && sum_fy) atomicAdd(&b.sum_y[ii], sum_fy);
     if (FULLCONV) {
         #pragma unroll
         for (int k = 0; k < 6; k++) {
@@ -181,6 +184,7 @@ __global__ void __launch_bounds__(PV_THREADS) k_preview(DevBatch b, jsgpu_previe
             if (v) atomicAdd(&o->cc_histo[0][0] + i, v);
         }
         for (uint32_t i = threadIdx.x; i < JSGPU_Y_HISTO_BINS; i += PV_THREADS) { const uint32_t v = sh.yh[i]; if (v) atomicAdd(&o->y_histo[i], v); }
+    }
     }
 }
 
@@ -252,7 +256,7 @@ int js_launch_preview(const DevBatch& b, const jsgpu_preview& pv, jsgpu_colour_s
     uint32_t per_img = (uint32_t)((sm_count * 8 + b.nimg - 1) / b.nimg);
     if (per_img > max_hp) per_img = max_hp;
     if (per_img < 1) per_img = 1;
-    const dim3 grid(per_img, b.nimg);
+    const dim3 grid(per_img, b.nimg < 65535u ? b.nimg : 65535u);
     int n = 0;
     if (full && hist) k_preview<true, true><<<grid, PV_THREADS, 0, s>>>(b, pv, st, rowclip);
     else if (full)    k_preview<true, false><<<grid, PV_THREADS, 0, s>>>(b, pv, st, rowclip);
