@@ -738,7 +738,7 @@ __global__ void __launch_bounds__(JS_HUFF_WARPS * 32) k_huff_warp(DevBatch b)
                         uint32_t nat = q >> 16;
                         int dcdiff = 0;
                         if (nat == 0) dcdiff = cf;
-                        else if (lane == (nat >> 1)) acc = (nat & 1) ? __byte_perm(acc, (uint32_t)cf, 0x5410) : __byte_perm(acc, (uint32_t)cf, 0x3254);
+                        else if (want_ac && lane == (nat >> 1)) acc = (nat & 1) ? __byte_perm(acc, (uint32_t)cf, 0x5410) : __byte_perm(acc, (uint32_t)cf, 0x3254);   // a DC symbol with a run nibble stores an AC value: none in DC-only mode (the reference runs no IDCT there)
                         dc = (int)(short)(dc + dcdiff);
                         pos = 1 + run;
                     }
@@ -999,7 +999,8 @@ __global__ void __launch_bounds__(LN_WARPS * 32, 3) k_huff_lane(DevBatch b)
                             const int cf = (int)(short)(val * (int)(q & 0xFFFF));
                             const uint32_t nat = q >> 16;
                             int dcdiff = 0;
-                            if (nat == 0) dcdiff = cf; else *reinterpret_cast<uint16_t*>(myrow + nat * 2) = (uint16_t)cf;
+                            if (nat == 0) dcdiff = cf;
+                            else if (want_ac) *reinterpret_cast<uint16_t*>(myrow + nat * 2) = (uint16_t)cf;    // run-nibble DC symbol: an AC value (none in DC-only mode)
                             dc = (int)(short)(dc + dcdiff);
                             pos = 1 + run;
                         }

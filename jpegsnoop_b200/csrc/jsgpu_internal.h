@@ -62,6 +62,7 @@ struct DevImage {
     uint32_t H[3], V[3], eh[3], ev[3];
     uint32_t slot_dc[3], slot_ac[3];// LUT slot per component
     uint32_t tab_sig;               // ns, slots and DQT selectors packed: equal (table_set, tab_sig) <=> same staged decode tables
+                                    // (not the same MCU layout: sampling factors and precision are not in it, k_ph_sync restages those per image)
     uint32_t dqt[3];
     uint32_t table_set;
     uint32_t file_pos;              // file offset of scan_off

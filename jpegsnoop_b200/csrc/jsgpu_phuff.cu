@@ -27,28 +27,34 @@ struct PhShared {
     uint8_t  blk_c[PH_MAX_BPM];
 };
 
-// Stage the distinct (class, Th) tables the image selects, exactly as the lane kernel lays them out.
+// The image's MCU layout (thread 0): which staged table every block of an MCU decodes with, its component, the blocks per
+// MCU and the precision's divide.  It depends on the sampling factors and the precision, which (table_set, tab_sig) does not
+// capture: images that share their staged tables can still differ here.
+__device__ __forceinline__ void ph_layout(PhShared& sh, const DevImage& im)
+{
+    uint32_t n = 0;
+    for (uint32_t c = 0; c < im.ns; c++) for (uint32_t cls = 0; cls < 2; cls++) {
+        const uint32_t slot = cls ? im.slot_ac[c] : im.slot_dc[c];
+        uint32_t j = 0;
+        while (j < n && sh.lslot[j] != slot) j++;
+        if (j == n) sh.lslot[n++] = slot;
+        sh.li[c * 2 + cls] = j;
+    }
+    sh.nl = n;
+    uint32_t bi = 0;
+    for (uint32_t c = 0; c < im.ns; c++)
+        for (uint32_t q = 0; q < im.H[c] * im.V[c] && bi < PH_MAX_BPM; q++, bi++) {
+            sh.blk_dc[bi] = (uint16_t)(sh.li[c * 2] * JS_LANE_TAB); sh.blk_ac[bi] = (uint16_t)(sh.li[c * 2 + 1] * JS_LANE_TAB); sh.blk_c[bi] = (uint8_t)c;
+        }
+    sh.bpm = bi;
+    sh.pshift = (im.precision > 8) ? im.precision - 8 : 0;
+}
+
+// Stage the distinct (class, Th) tables the image selects, exactly as the lane kernel lays them out, and its MCU layout.
 __device__ __forceinline__ void ph_stage(PhShared& sh, uint16_t* lutb, const DevImage& im, const DevTableSet* ts)
 {
     __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t n = 0;
-        for (uint32_t c = 0; c < im.ns; c++) for (uint32_t cls = 0; cls < 2; cls++) {
-            const uint32_t slot = cls ? im.slot_ac[c] : im.slot_dc[c];
-            uint32_t j = 0;
-            while (j < n && sh.lslot[j] != slot) j++;
-            if (j == n) sh.lslot[n++] = slot;
-            sh.li[c * 2 + cls] = j;
-        }
-        sh.nl = n;
-        uint32_t bi = 0;
-        for (uint32_t c = 0; c < im.ns; c++)
-            for (uint32_t q = 0; q < im.H[c] * im.V[c] && bi < PH_MAX_BPM; q++, bi++) {
-                sh.blk_dc[bi] = (uint16_t)(sh.li[c * 2] * JS_LANE_TAB); sh.blk_ac[bi] = (uint16_t)(sh.li[c * 2 + 1] * JS_LANE_TAB); sh.blk_c[bi] = (uint8_t)c;
-            }
-        sh.bpm = bi;
-        sh.pshift = (im.precision > 8) ? im.precision - 8 : 0;
-    }
+    if (threadIdx.x == 0) ph_layout(sh, im);
     __syncthreads();
     const uint32_t nl = sh.nl;
     for (uint32_t j = 0; j < nl; j++) {
@@ -92,7 +98,7 @@ __global__ void __launch_bounds__(PH_THREADS, 5) k_ph_sync(DevBatch b, uint32_t 
     extern __shared__ __align__(16) uint8_t ph_smem[];
     PhShared& sh = *reinterpret_cast<PhShared*>(ph_smem);
     uint16_t* const lutb = reinterpret_cast<uint16_t*>(ph_smem + sizeof(PhShared));
-    uint32_t cur_sig = 0xffffffffu, cur_set = 0xffffffffu, nchg = 0;
+    uint32_t cur_sig = 0xffffffffu, cur_set = 0xffffffffu, cur_img = 0xffffffffu, nchg = 0;
     const uint32_t* const lin = b.ph_list[(round + 1) & 1]; const uint32_t* const nin = b.ph_nl[(round + 1) & 1];    // written by round - 1
     uint32_t* const lout = b.ph_list[round & 1]; uint32_t* const nout = b.ph_nl[round & 1];
     for (uint32_t it = blockIdx.x; it < b.nvitems; it += gridDim.x) {
@@ -100,9 +106,14 @@ __global__ void __launch_bounds__(PH_THREADS, 5) k_ph_sync(DevBatch b, uint32_t 
         const DevImage& im = b.img[item.x];
         uint32_t nlist = 0;
         if (MODE == 2) { nlist = nin[item.x]; if (item.y >= nlist) continue; }     // CTA-uniform
-        if (im.tab_sig != cur_sig || im.table_set != cur_set) {
+        if (im.tab_sig != cur_sig || im.table_set != cur_set) {          // other decode tables: stage them and the layout
             ph_stage(sh, lutb, im, b.tables + im.table_set);
-            cur_sig = im.tab_sig; cur_set = im.table_set;
+            cur_sig = im.tab_sig; cur_set = im.table_set; cur_img = item.x;
+        } else if (item.x != cur_img) {                                    // same tables, another image: its own MCU layout
+            __syncthreads();
+            if (threadIdx.x == 0) ph_layout(sh, im);
+            __syncthreads();
+            cur_img = item.x;
         }
         uint32_t slot = item.y + threadIdx.x;
         if (MODE == 2) { if (slot >= nlist) continue; slot = lin[im.ph_first + slot]; }

@@ -16,10 +16,17 @@ from mini_jpeg import ZZ, BitWriter, bits_from_lengths, canonical_codes, _seg
 
 # --- Huffman tables --------------------------------------------------------------------------------------------------
 
-def dc_table(long_codes=True):
-    """DC sizes 0..15; with long_codes the sizes 14 and 15 have 16-bit codes (a 16 + 15 = 31-bit step)."""
-    lengths = [2, 3, 3, 3, 3, 3, 4, 5, 6, 7, 8, 9, 12, 12] + ([16, 16] if long_codes else [13, 13])
-    return bits_from_lengths(lengths), list(range(16))
+# DC symbols with a run nibble: (r << 4) | s carries a size-s value that lands at zig-zag position r (ImgDecode.cpp
+# DecodeIdctSet stores it at num_coeffs + zrl); the block goes on at 1 + r and its DC difference is 0.
+DC_RUN_SYMBOLS = [(r << 4) | (r * 7 % 15 + 1) for r in range(1, 16)]
+
+
+def dc_table(long_codes=True, runs=False):
+    """DC sizes 0..15; with long_codes the sizes 14 and 15 have 16-bit codes (a 16 + 15 = 31-bit step).  runs adds the
+    DC_RUN_SYMBOLS behind 14-bit codes."""
+    extra = DC_RUN_SYMBOLS if runs else []
+    lengths = [2, 3, 3, 3, 3, 3, 4, 5, 6, 7, 8, 9, 12, 12] + [14] * len(extra) + ([16, 16] if long_codes else [13, 13])
+    return bits_from_lengths(lengths), list(range(14)) + extra + [14, 15]
 
 
 def ac_table(long_codes=True, variant=0):
@@ -63,7 +70,8 @@ def _mcu_order(W, H, samp):
     return order
 
 
-def encode_coefs(blocks, W, H, samp, qtabs, qsel, precision=8, dri=0, long_codes=True, force_pq16=False):
+def encode_coefs(blocks, W, H, samp, qtabs, qsel, precision=8, dri=0, long_codes=True, force_pq16=False,
+                 shared_tables=False, dc_runs=None, trace=None):
     """A JPEG whose scan carries exactly these coefficients.
 
     blocks: one int array per component, (block rows, block cols, 64) in natural order, holding the values as written
@@ -72,6 +80,13 @@ def encode_coefs(blocks, W, H, samp, qtabs, qsel, precision=8, dri=0, long_codes
     samp:   (H, V) per component (one entry = greyscale).
     qtabs:  quantisation tables, 64 values 1..65535 in natural order; a table is written with Pq = 1 when an entry
             exceeds 255 or force_pq16 is set.  qsel: table index per component.
+    shared_tables: every component uses DC/AC table 0 (else luma 0, chroma 1).
+    dc_runs: per component, block-grid shaped run nibbles r (0..15): a block with r > 0 writes its zig-zag value r with the
+            DC symbol (r << 4) | size (the DC table then holds DC_RUN_SYMBOLS); its DC must equal the previous block's and
+            its zig-zag values 1 .. r-1 must be 0.  `expected` does not model this.
+    trace:  a list that receives, per restart interval, a dict of the unstuffed bit position of every MCU start
+            ("mcu_bits") and block start ("blk_bits", per MCU), the reference's int16 DC predictors at every MCU start
+            ("dc", per MCU one value per component) and the interval's unstuffed length in bits ("nbits", before padding).
     Returns (jpeg bytes, spec): spec is what `expected` needs."""
     ncomp = len(samp)
     assert ncomp in (1, 3) and precision in (8, 12)
@@ -84,39 +99,65 @@ def encode_coefs(blocks, W, H, samp, qtabs, qsel, precision=8, dri=0, long_codes
     qtabs = [np.asarray(q, np.int64) for q in qtabs]
     for q in qtabs:
         assert q.shape == (64,) and q.min() >= 1 and q.max() <= 65535
-    ntab = 1 if ncomp == 1 else 2
-    dc_tabs = [dc_table(long_codes)] * ntab
+    ntab = 1 if (ncomp == 1 or shared_tables) else 2
+    dc_tabs = [dc_table(long_codes, runs=dc_runs is not None)] * ntab
     ac_tabs = [ac_table(long_codes, variant=t) for t in range(ntab)]
     dcc = [canonical_codes(*t) for t in dc_tabs]; acc = [canonical_codes(*t) for t in ac_tabs]
     zz = [b[..., ZZ] for b in blocks]                         # zig-zag order, so a block's symbols are a left-to-right walk
     bw = BitWriter(); out = bytearray(); pred = [0] * ncomp; rst = 0
+    div = 1 << (precision - 8)
+    cdiv = lambda a: -(-a // div) if a < 0 else a // div
+    i16 = lambda a: ((a + 32768) & 0xFFFF) - 32768
+    nbits = [0]; dcp = [0] * ncomp                          # bits of the current interval; the reference's short predictors
+    new_iv = lambda: {"mcu_bits": [], "blk_bits": [], "dc": [], "nbits": 0}
+    cur = new_iv()
+
+    def put(code, length):
+        bw.put(code, length); nbits[0] += length
 
     def put_val(code_len, a, s):
         code, length = code_len
-        bw.put((code << s) | ((a if a > 0 else a + (1 << s) - 1) & ((1 << s) - 1)), length + s)
+        put((code << s) | ((a if a > 0 else a + (1 << s) - 1) & ((1 << s) - 1)), length + s)
 
     for n, mcu in enumerate(_mcu_order(W, H, samp)):
         if dri and n and n % dri == 0:
+            cur["nbits"] = nbits[0]
+            if trace is not None:
+                trace.append(cur)
             bw.flush(); out += bw.out; out += bytes([0xFF, 0xD0 + (rst & 7)]); rst += 1
-            bw = BitWriter(); pred = [0] * ncomp
+            bw = BitWriter(); pred = [0] * ncomp; nbits[0] = 0; dcp = [0] * ncomp; cur = new_iv()
+        cur["mcu_bits"].append(nbits[0]); cur["blk_bits"].append([]); cur["dc"].append(list(dcp))
         for c, br, bc in mcu:
-            t = 0 if c == 0 else 1
+            cur["blk_bits"][-1].append(nbits[0])
+            t = 0 if (c == 0 or shared_tables) else 1
             z = zz[c][br, bc]
             diff = int(z[0]) - pred[c]; pred[c] = int(z[0])
             assert abs(diff) <= 32767, ("DC difference needs more than 15 bits", c, br, bc, diff)
-            s = abs(diff).bit_length()
-            put_val(dcc[t][s], diff, s)
-            nz = np.flatnonzero(z[1:]) + 1
+            r = int(dc_runs[c][br, bc]) if dc_runs is not None else 0
             k = 1
+            if r:
+                assert diff == 0 and not z[1:r].any() and z[r], ("a DC run symbol needs DC difference 0 and zig-zag values", c, br, bc)
+                a = int(z[r]); s = abs(a).bit_length()
+                assert (r << 4) | s in dcc[t], ("no DC run symbol", hex((r << 4) | s))
+                put_val(dcc[t][(r << 4) | s], a, s)
+                k = r + 1
+            else:
+                s = abs(diff).bit_length()
+                put_val(dcc[t][s], diff, s)
+                dcp[c] = i16(dcp[c] + i16(cdiv(diff) * int(qtabs[qsel[c]][0])))
+            nz = np.flatnonzero(z[k:]) + k
             for p in nz.tolist():
                 run = p - k
                 while run > 15:
-                    bw.put(*acc[t][0xF0]); run -= 16
+                    put(*acc[t][0xF0]); run -= 16
                 a = int(z[p]); s = abs(a).bit_length()
                 put_val(acc[t][(run << 4) | s], a, s)
                 k = p + 1
             if k < 64:
-                bw.put(*acc[t][0x00])
+                put(*acc[t][0x00])
+    cur["nbits"] = nbits[0]
+    if trace is not None:
+        trace.append(cur)
     bw.flush(); out += bw.out
     f = bytearray(b"\xFF\xD8")
     for i, q in enumerate(qtabs):
@@ -130,7 +171,7 @@ def encode_coefs(blocks, W, H, samp, qtabs, qsel, precision=8, dri=0, long_codes
         f += _seg(0xC4, bytes([0x10 | i]) + bytes(ac_tabs[i][0]) + bytes(ac_tabs[i][1]))
     if dri:
         f += _seg(0xDD, dri.to_bytes(2, "big"))
-    f += _seg(0xDA, bytes([ncomp]) + b"".join(bytes([c + 1, 0x00 if c == 0 else 0x11]) for c in range(ncomp)) + bytes([0, 63, 0]))
+    f += _seg(0xDA, bytes([ncomp]) + b"".join(bytes([c + 1, 0x00 if (c == 0 or shared_tables) else 0x11]) for c in range(ncomp)) + bytes([0, 63, 0]))
     spec = dict(blocks=blocks, W=W, H=H, samp=tuple(tuple(s) for s in samp), qtabs=qtabs, qsel=tuple(qsel), precision=precision, dri=dri)
     return bytes(f + out + b"\xFF\xD9"), spec
 

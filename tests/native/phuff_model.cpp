@@ -122,9 +122,38 @@ void walk(const DevTableSet& ts, const Geo& g, const uint32_t* w, uint32_t ulen,
 
 }  // namespace
 
+// Every interval's MCU start bits and DC predictors by the sequential walk, concatenated (at most cap MCUs); ulen[k] =
+// unstuffed length of interval k in bytes (at most nseg_cap intervals).  Returns the number of MCUs walked, or < 0.
+extern "C" int phm_walk(const jsgpu_tables* tabs, const jsgpu_image_desc* desc, const uint8_t* scan, uint64_t n,
+                        uint32_t* mcu_bit, int16_t* dc, uint32_t cap, uint32_t* ulen, uint32_t nseg_cap)
+{
+    Geo g;
+    if (!make_geo(*desc, g)) return -1;
+    static DevTableSet ts;
+    build_table_set(*tabs, ts);
+    std::vector<Interval> iv; std::vector<uint8_t> ub;
+    unstuff(scan, n, g, iv, ub);
+    uint32_t m = 0;
+    for (uint32_t k = 0; k < g.nseg; k++) {
+        Truth t;
+        walk(ts, g, reinterpret_cast<const uint32_t*>(ub.data() + iv[k].uoff), iv[k].ulen, std::min(g.ri, g.nmcu - k * g.ri), t);
+        if (k < nseg_cap) ulen[k] = iv[k].ulen;
+        for (uint32_t i = 0; i < t.nmcu_done && m < cap; i++, m++) {
+            mcu_bit[m] = t.mcu_bit[i]; dc[m * 3] = t.dc[i * 3]; dc[m * 3 + 1] = t.dc[i * 3 + 1]; dc[m * 3 + 2] = t.dc[i * 3 + 2];
+        }
+    }
+    return (int)m;
+}
+
 // order: 0 = descending slot order (pure "previous round" reads), 1 = ascending, 2 = pseudo-random
 // out[0] = mismatches, out[1] = fix rounds until settled, out[2] = slots in use, out[3] = virtual intervals,
-// out[4] = slots whose guess was already right, out[5] = MCUs covered
+// out[4] = slots whose guess was already right, out[5] = MCUs covered.  What the settled exit states reach (a slot's exit
+// state is where its decoder stops: the first symbol start at or after the slot's end):
+// out[6] = slots with no MCU start, out[7] = exits inside an MCU (block != 0), out[8] = exits inside a block (zig-zag != 0),
+// out[9] = exits past the slot's end, out[10] = the largest overshoot in bits, out[11] = exits whose next symbol is an EOB,
+// out[12] = the most MCU starts in one slot, out[13] = bit mask of the exit block indices 0..31, out[14] = ... 32..63,
+// out[15] = mask of exit zig-zag indices 0..31, out[16] = ... 32..63, out[17] = slots that settled only after PH_MAX_ROUNDS
+// fix rounds (their exit state last changed in a later round), out[18] = fix rounds that changed a slot after PH_MAX_ROUNDS
 extern "C" int phm_check(const jsgpu_tables* tabs, const jsgpu_image_desc* desc, const uint8_t* scan, uint64_t n, int order, uint32_t* out)
 {
     Geo g;
@@ -168,11 +197,12 @@ extern "C" int phm_check(const jsgpu_tables* tabs, const jsgpu_image_desc* desc,
     if (order == 2) { uint32_t r = 12345; for (uint32_t i = nslots; i > 1; i--) { r = r * 1664525u + 1013904223u; std::swap(ord[i - 1], ord[(r >> 8) % i]); } }
     for (uint32_t i = 0; i < nslots; i++) ph_guess_slot(t, sg, ub.data(), a, ord[i]);
     const std::vector<unsigned long long> xguess = x;
-    uint32_t rounds = 0;
+    uint32_t rounds = 0, late_rounds = 0;
     for (uint32_t r = 1; r < 100000; r++) {
         uint32_t nchg = 0;
         for (uint32_t i = 0; i < nslots; i++) nchg += ph_fix_slot(t, sg, ub.data(), a, ord[i], r) ? 1 : 0;
         rounds = r;
+        if (r > PH_MAX_ROUNDS && nchg) late_rounds++;
         if (!nchg) break;
     }
     uint4 run = make_uint4(0, 0, 0, 0);                       // k_ph_scan
@@ -212,5 +242,27 @@ extern "C" int phm_check(const jsgpu_tables* tabs, const jsgpu_image_desc* desc,
         if (iv[k].ulen && next_m[k] != k * g.ri + cntk) { bad++; if (bad < 5) fprintf(stderr, "interval %u: virtual intervals end at MCU %u, expected %u\n", k, next_m[k], k * g.ri + cntk); }
     }
     out[0] = bad; out[1] = rounds; out[2] = used; out[3] = nv; out[4] = guessed; out[5] = covered;
+    // ---- what the settled exit states reach ---------------------------------------------------------------------------
+    for (uint32_t i = 6; i < 19; i++) out[i] = 0;
+    for (uint32_t s = 0; s < nslots; s++) {
+        if (kk[s] == PH_NONE || x[s] == PH_DEAD) continue;
+        const uint32_t k = kk[s], i = s - ph_slot_base(st[k], k), end = ul[k] * 8u;
+        const uint32_t lim = std::min((i + 1) << PH_SUB_SHIFT, end);
+        const uint32_t pos = ph_pos(x[s]), blk = ph_blk(x[s]), zz = ph_zz(x[s]);
+        if (cnt[s].x == 0) out[6]++;
+        out[12] = std::max(out[12], cnt[s].x);
+        if (pos >= end) continue;                                   // the interval's end: no state inside the data
+        if (blk) out[7]++;
+        if (zz) out[8]++;
+        if (pos > lim) { out[9]++; out[10] = std::max(out[10], pos - lim); }
+        out[13 + (blk >> 5)] |= 1u << (blk & 31);
+        out[15 + (zz >> 5)] |= 1u << (zz & 31);
+        if (zz) {
+            const uint32_t e = lookup(ts, g.sac[bc[blk]], peek(reinterpret_cast<const uint32_t*>(ub.data() + iv[k].uoff), pos));
+            if (e && (e & 0xFF) == 0) out[11]++;
+        }
+        if (ver[s] > PH_MAX_ROUNDS) out[17]++;
+    }
+    out[18] = late_rounds;
     return 0;
 }

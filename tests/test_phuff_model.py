@@ -46,7 +46,7 @@ def test_virtual_intervals_match_a_sequential_walk(model, order):
     for name, j in _cases():
         t, d, start = parse_jpeg(j)
         scan = np.frombuffer(j, np.uint8)[start:].copy()
-        out = np.zeros(8, np.uint32)
+        out = np.zeros(32, np.uint32)
         r = model.phm_check(C.byref(t), C.byref(d), scan.ctypes.data, scan.size, order, out.ctypes.data)
         assert r == 0, (name, r)
         bad, rounds, used, nv, guessed, covered = [int(v) for v in out[:6]]
