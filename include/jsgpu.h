@@ -98,8 +98,8 @@ typedef struct {
     int32_t huff_kernel;    /* 0 = auto (3 for images with long restart intervals, else 2 or 1 by the
                                number of intervals), 1 = one warp per restart interval, 2 = one lane
                                per restart interval, 3 = self-synchronising passes for long intervals */
-    int32_t idct_kernel;    /* 0 = auto, 1 = simple reference kernels, 2 = fused tile kernel with
-                               TMA-staged coefficients, 3 = fused tile kernel with plain loads    */
+    int32_t idct_kernel;    /* 1 = simple reference kernels; 0 (auto), 2 and 3 all = fused tile
+                               kernel where it applies, simple kernels elsewhere                   */
     int32_t want_histo;     /* accumulate m_anDhtHisto (ImgDecode.cpp:1190-1191); default 1      */
     int32_t want_mcu_map;   /* build m_pMcuFileMap (ImgDecode.cpp:3229); default 1               */
     int32_t device_markers; /* 1 = find RSTn/end-of-scan on the GPU (default), 0 = host walk      */

@@ -45,7 +45,7 @@ struct jsgpu_ctx {
     // device state
     DevBuf d_ctab; bool have_ctab = false;
     DevBuf d_li, d_lf, d_sym, d_tables, d_img, d_items, d_litems, d_tiles, d_ubits, d_seg64, d_ph, d_rowtab, d_ex;
-    bool sym_ok = false, baked_ok = false, bakedf_ok = false; int tab_mode = 0;
+    bool sym_ok = false, baked_ok = false, bakedf_ok = false, tab_baked = false;
     DevBuf d_bits, d_seg, d_coef, d_mcubits, d_pix, d_dib, d_blk, d_mcumap, d_histo, d_stats, d_misc;
     uint32_t nsets = 0;
     std::vector<std::array<uint32_t, JS_NSLOT>> set_l2;   // per table set and slot: second-level entries used (0xffffffff = overflowed)
@@ -57,7 +57,6 @@ struct jsgpu_ctx {
     uint64_t bits_len = 0, pix_total = 0, dib_total = 0, blk_total = 0, mcu_total = 0, coef_rows = 0;
     uint64_t max_scan_len = 0, ubits_total = 0, ph_total = 0, rt_total = 0;
     uint32_t nseg_np = 0, n_psync = 0, max_cs = 0; uint64_t cs_total = 0;
-    alignas(64) unsigned char tmap[128]; bool tmap_ok = false;
     uint32_t n_nonstd = 0, n_std = 0;
     int launches = 0;
     // host copies of the configuration, replayed into the chunk contexts of jsgpu_decode_batch_host
@@ -213,17 +212,16 @@ int jsgpu_set_idct_tables(jsgpu_ctx* ctx, const int32_t* li, const float* lf)
     ctx->baked_ok = js_idct_baked_matches(li) != 0;
     ctx->bakedf_ok = js_idctf_baked_matches(lf) != 0;
     ctx->h_li.assign(li, li + 64 * 64); ctx->h_lf.assign(lf, lf + 64 * 64);
-    {   // table source of the LDG tile kernel: env override for experiments, else immediates when the baked copy matches
+    {   // the integer tile kernel takes its table as immediates when the baked copy matches, else from shared memory;
+        // JSGPU_IDCT_TABLE=0 forces the shared-memory table (tests)
         const char* e = getenv("JSGPU_IDCT_TABLE");
-        ctx->tab_mode = e ? atoi(e) : (ctx->baked_ok ? 2 : 0);
-        if (ctx->tab_mode == 2 && !ctx->baked_ok) ctx->tab_mode = 0;
+        ctx->tab_baked = ctx->baked_ok && !(e && atoi(e) == 0);
     }
     cudaError_t e1 = ctx->d_li.reserve(64 * 64 * 4), e2 = ctx->d_lf.reserve(64 * 64 * 4), e3 = ctx->d_sym.reserve(sizeof(IdctSym));
     if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess) { delete sym; return fail(ctx, JSGPU_ENOMEM, "idct table allocation failed"); }
     cudaMemcpyAsync(ctx->d_li.p, li, 64 * 64 * 4, cudaMemcpyHostToDevice, ctx->stream);
     cudaMemcpyAsync(ctx->d_lf.p, lf, 64 * 64 * 4, cudaMemcpyHostToDevice, ctx->stream);
     cudaMemcpyAsync(ctx->d_sym.p, sym, sizeof(IdctSym), cudaMemcpyHostToDevice, ctx->stream);
-    js_upload_idct_constants(sym, ctx->stream);
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     delete sym;
     if (e != cudaSuccess) return fail(ctx, JSGPU_ECUDA, "idct table upload failed: %s", cudaGetErrorString(e));
@@ -448,7 +446,8 @@ int jsgpu_batch_begin(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32_t n, 
     CK(ctx->d_tiles.reserve(sizeof(uint4) * std::max<size_t>(tiles.size(), 1)));
     CK(ctx->d_seg64.reserve(8 * (size_t)seg + 16));
     CK(ctx->d_seg.reserve(sizeof(uint32_t) * ((7 + JS_STUFF_LIST) * (size_t)seg + 2 * (size_t)n + 16)));
-    CK(ctx->d_coef.reserve(rows * 128 + 4096));      // + slack: a TMA box may start at the last rows and spans 8
+    CK(ctx->d_coef.reserve(rows * 128 + 4096));      // + 4096 spare bytes: no kernel addresses them (every row index is bounded by
+                                                     // its plane); kept so that the pool sizes stay as measured
     CK(ctx->d_mcubits.reserve(mcu * 4 + 16));
     CK(ctx->d_pix.reserve(pix * 2 * 3 + 64));
     CK(ctx->d_dib.reserve(dib + 64));
@@ -495,7 +494,6 @@ int jsgpu_batch_begin(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32_t n, 
     }
     b.tiles = (const uint4*)ctx->d_tiles.p; b.ntiles = (uint32_t)tiles.size(); b.tile_plane_bytes = plane_bytes;
     for (int k = 0; k < 3; k++) { b.tcls_first[k] = tcls_first[k]; b.tcls_count[k] = tcls_count[k]; }
-    ctx->tmap_ok = (js_make_coef_tensor_map(ctx->tmap, ctx->d_coef.p, rows + 8) == 0);
     b.items = (const uint2*)ctx->d_items.p; b.nitems = (uint32_t)n_it;
     b.items_np = b.items + n_it; b.nitems_np = (uint32_t)items_np.size();
     b.coef = (int16_t*)ctx->d_coef.p; b.mcu_bitpos = (uint32_t*)ctx->d_mcubits.p;
@@ -679,19 +677,17 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx)
     }
     CK(cudaEventRecord(ctx->ev[2], s));
     {
-        // fused tile kernel: integer IDCT, standard sampling layouts, decomposable table; everything
-        // else (float IDCT, exotic sampling, a libm whose table does not decompose) takes the simple kernels
-        const bool fused = (ctx->opt.idct_kernel != 1) && ctx->opt.idct_mode == 0 && ctx->sym_ok && b.ntiles > 0;
-        // idct_kernel: 2 = TMA-staged tile kernel, 0/3 = tile kernel with per-lane vector loads (the default)
-        if (fused && ctx->opt.idct_kernel == 2 && ctx->tmap_ok) launches += js_launch_idct_tma(b, (const IdctSym*)ctx->d_sym.p, (const ColorTabs*)ctx->d_ctab.p, ctx->tmap, ctx->sm_count, s);
-        else if (fused) launches += js_launch_idct_fused(b, (const IdctSym*)ctx->d_sym.p, (const ColorTabs*)ctx->d_ctab.p, ctx->sm_count, ctx->tab_mode, s);
-        // float IDCT (the reference's default build): fused tile kernel with the float table as immediates, when that table
-        // is the host's, bit for bit; idct_kernel = 1 forces the literal kernels
-        const bool fusedf = (ctx->opt.idct_kernel != 1) && ctx->opt.idct_mode == 1 && ctx->bakedf_ok && b.ntiles > 0;
-        if (fusedf) launches += js_launch_idct_fused_float(b, (const ColorTabs*)ctx->d_ctab.p, ctx->sm_count, s);
-        if (!(fused || fusedf) || ctx->n_nonstd > 0) {
-            DevBatch bs = b; bs.simple_only_nonstd = (fused || fusedf) ? 1 : 0;
-            launches += js_launch_idct_simple(bs, (const int32_t*)ctx->d_li.p, (const float*)ctx->d_lf.p, 0, 0, s);
+        // fused tile kernel for the images with standard sampling layouts, when the integer table decomposes (integer IDCT) or
+        // the float table is the baked one, bit for bit (float IDCT, the reference's default build); everything else (exotic
+        // sampling, a host table the tile kernel cannot use, idct_kernel = 1) takes the simple kernels
+        const bool flt = ctx->opt.idct_mode == 1;
+        const bool fused = ctx->opt.idct_kernel != 1 && b.ntiles > 0 && (flt ? ctx->bakedf_ok : ctx->sym_ok);
+        if (fused)
+            launches += js_launch_idct_fused(b, (const IdctSym*)ctx->d_sym.p, (const ColorTabs*)ctx->d_ctab.p, ctx->sm_count,
+                                             flt ? JS_TILE_FLOAT : ctx->tab_baked ? JS_TILE_INT_BAKED : JS_TILE_INT_SMEM, s);
+        if (!fused || ctx->n_nonstd > 0) {
+            DevBatch bs = b; bs.simple_only_nonstd = fused ? 1 : 0;
+            launches += js_launch_idct_simple(bs, (const int32_t*)ctx->d_li.p, (const float*)ctx->d_lf.p, s);
         }
     }
     CK(cudaEventRecord(ctx->ev[3], s));

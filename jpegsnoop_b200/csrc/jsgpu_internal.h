@@ -174,17 +174,14 @@ int js_launch_huffman_warp(const DevBatch& b, int sm_count, cudaStream_t s);
 int js_launch_huffman_lane(const DevBatch& b, int sm_count, cudaStream_t s);
 int js_launch_huffman_lane_vseg(const DevBatch& b, int sm_count, cudaStream_t s);   // over the virtual intervals the self-synchronising passes found
 int js_launch_selfsync(const DevBatch& b, int sm_count, cudaStream_t s);            // guess + fix rounds + scan (jsgpu_phuff.cu)
-int js_launch_idct_simple(const DevBatch& b, const int32_t* li, const float* lf, uint64_t total_blocks,
-                          uint64_t total_pix, cudaStream_t s);
+int js_launch_idct_simple(const DevBatch& b, const int32_t* li, const float* lf, cudaStream_t s);
 struct IdctSym; struct ColorTabs;
-int js_launch_idct_fused(const DevBatch& b, const IdctSym* sym, const ColorTabs* ctab, int sm_count, int tab_mode, cudaStream_t s);
+// phase 1 of the fused tile kernel (jsgpu_idct.cu): integer IDCT with the table in shared memory or as immediates, float IDCT
+enum JsTileIdct { JS_TILE_INT_SMEM, JS_TILE_INT_BAKED, JS_TILE_FLOAT };
+int js_launch_idct_fused(const DevBatch& b, const IdctSym* sym, const ColorTabs* ctab, int sm_count, JsTileIdct idct, cudaStream_t s);
 int js_idct_baked_matches(const int32_t* li);
 int js_idctf_baked_matches(const float* lf);
-int js_launch_idct_fused_float(const DevBatch& b, const ColorTabs* ctab, int sm_count, cudaStream_t s);   // float-IDCT build, fused (jsgpu_idctf.cu)
 int js_launch_build_color_tables(ColorTabs* t, cudaStream_t s);
-int js_upload_idct_constants(const IdctSym* host_sym, cudaStream_t s);
-int js_make_coef_tensor_map(void* out_tmap, void* coef, uint64_t rows);
-int js_launch_idct_tma(const DevBatch& b, const IdctSym* sym, const ColorTabs* ctab, const void* tmap_host, int sm_count, cudaStream_t s);
 int js_launch_exact(const DevBatch& b, int err_max, const jsgpu_detail& dtl, jsgpu_detail_dump* dump, uint32_t* scratch_histo, cudaStream_t s);       // damaged images, again, with the reference's semantics (jsgpu_exact.cu)
 int js_launch_export(const DevBatch& b, uint32_t image, int mode, uint8_t* out, uint64_t npx, int sm_count, cudaStream_t s);   // Export-to-TIFF sample array
 int js_launch_finalize_maps(const DevBatch& b, cudaStream_t s);     // MCU file map (independent of the IDCT)

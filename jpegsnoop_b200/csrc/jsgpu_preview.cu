@@ -11,6 +11,7 @@
 // reproduces the reference's "first YCC_CLIP_REPORT_MAX notes, and only those are counted" rule (:4372-4378) by walking, in
 // raster order, just the rows that have events.
 #include "jsgpu_internal.h"
+#include "jsgpu_ycc.cuh"
 
 #define FULL 0xffffffffu
 #define PV_THREADS 256
@@ -23,27 +24,12 @@ struct PvPix {                       // PixelCc (ImgDecode.h:186-216), the field
     uint32_t fr, fg, fb;             // nFinalR/G/B
 };
 
-__device__ __forceinline__ void pv_convert(float y, float cb, float cr, float& vr, float& vg, float& vb)
-{
-    // nValR = nValCr*(2-2*fConstRed)+nValY ... (:4289-4296 and :4118-4125), one IEEE rounding per operation (-ffp-contract=off)
-    const float cR = 0.299f, cG = 0.587f, cB = 0.114f;
-    const float kR = __fsub_rn(2.0f, __fmul_rn(2.0f, cR)), kB = __fsub_rn(2.0f, __fmul_rn(2.0f, cB));
-    vr = __fadd_rn(__fmul_rn(cr, kR), y);
-    vb = __fadd_rn(__fmul_rn(cb, kB), y);
-    vg = __fdiv_rn(__fsub_rn(__fsub_rn(y, __fmul_rn(cB, vb)), __fmul_rn(cR, vr)), cG);
-    vr = __fadd_rn(vr, 128.f); vb = __fadd_rn(vb, 128.f); vg = __fadd_rn(vg, 128.f);
-}
-
 // ConvertYCCtoRGBFastFloat (ImgDecode.cpp:4086-4139)
 __device__ __forceinline__ void pv_fast(PvPix& p)
 {
-    int y = p.pre_y >> 3, cb = p.pre_cb >> 3, cr = p.pre_cr >> 3;
-    y = max(-128, min(127, y)); cb = max(-128, min(127, cb)); cr = max(-128, min(127, cr));
-    p.fy = (uint32_t)(y + 128) & 0xFF; p.fcb = (uint32_t)(cb + 128) & 0xFF; p.fcr = (uint32_t)(cr + 128) & 0xFF;
-    float vr, vg, vb; pv_convert((float)y, (float)cb, (float)cr, vr, vg, vb);
-    p.fr = (vr < 0.f) ? 0u : (vr > 255.f) ? 255u : (uint32_t)(int)vr;
-    p.fg = (vg < 0.f) ? 0u : (vg > 255.f) ? 255u : (uint32_t)(int)vg;
-    p.fb = (vb < 0.f) ? 0u : (vb > 255.f) ? 255u : (uint32_t)(int)vb;
+    const YccFast o = ycc_fast(p.pre_y, p.pre_cb, p.pre_cr);
+    p.fy = (uint32_t)(o.y + 128); p.fcb = (uint32_t)(o.cb + 128); p.fcr = (uint32_t)(o.cr + 128);
+    p.fr = o.r; p.fg = o.g; p.fb = o.b;
 }
 
 // ConvertYCCtoRGB without its bookkeeping (:4229-4325): ranging (C division, truncating), YCC clip, conversion, RGB clip
@@ -52,7 +38,7 @@ __device__ __forceinline__ void pv_full(PvPix& p)
     p.rng_y = (p.pre_y + 1024) / 8; p.rng_cb = (p.pre_cb + 1024) / 8; p.rng_cr = (p.pre_cr + 1024) / 8;
     const int y = max(0, min(255, p.rng_y)), cb = max(0, min(255, p.rng_cb)), cr = max(0, min(255, p.rng_cr));
     p.fy = (uint32_t)y; p.fcb = (uint32_t)cb; p.fcr = (uint32_t)cr;
-    float vr, vg, vb; pv_convert((float)(y - 128), (float)(cb - 128), (float)(cr - 128), vr, vg, vb);
+    float vr, vg, vb; ycc_float_core((float)(y - 128), (float)(cb - 128), (float)(cr - 128), vr, vg, vb);
     p.pr = __float2int_rz(vr); p.pg = __float2int_rz(vg); p.pb = __float2int_rz(vb);
     p.fr = (uint32_t)max(0, min(255, p.pr)); p.fg = (uint32_t)max(0, min(255, p.pg)); p.fb = (uint32_t)max(0, min(255, p.pb));
 }

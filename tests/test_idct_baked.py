@@ -1,5 +1,5 @@
 """CPU test of the build-time IDCT table generator (jpegsnoop_b200/csrc/tools/gen_idct_table.cpp): the literal
-multiply-add / butterfly / correction sequence compiled into k_idct_tile<2,*> equals the plain integer sums of the
+multiply-add / butterfly / correction sequence compiled into k_idct_tile<JS_TILE_INT_BAKED,*> equals the plain integer sums of the
 reference's table, and the table itself equals the one the compiled reference computes (golden fixture)."""
 import os
 import subprocess

@@ -5,7 +5,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(
 import numpy as np
 from jpegsnoop_b200 import BatchDecoder, synth
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 16
-variants = [tuple(int(x) for x in v.split(",")) for v in sys.argv[2:]] or [(1, 1), (2, 2)]
+variants = [tuple(int(x) for x in v.split(",")) for v in sys.argv[2:]] or [(1, 1), (2, 3)]
 t = time.time()
 specs = [dict(width=1920, height=1080, subsampling="420", quality=85, restart_interval=4, optimize=False, seed=2000 + i) for i in range(n)]
 buf, offs = synth.encode_batch(specs)
