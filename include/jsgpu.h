@@ -307,9 +307,13 @@ int jsgpu_batch_colour_stats(jsgpu_ctx* ctx, uint32_t image, jsgpu_colour_stats*
 
 /* --- "Detailed Decode" of chosen MCUs (CimgDecode::SetDetailVlc, ImgDecode.cpp:4898; DecodeScanCompPrint :1859-2090) ------
  * For `len` MCUs from (mcu_x, mcu_y) of image `image` the reference prints every Huffman symbol (ReportVlc :2152-2232) and each
- * block's coefficient matrix (ReportDctMatrix :2104-2131).  The serial reference-semantics walk (the one damaged images take)
- * collects them; jsgpu_batch_detail returns them after jsgpu_batch_decode.  In DC-only mode the printed MCUs are decoded in full
- * (AC + IDCT), as DecodeScanCompPrint does. */
+ * block's coefficient matrix (ReportDctMatrix :2104-2131), whatever `len` is.  For an image whose status word is 0 one GPU thread
+ * per MCU of the range decodes it from the MCU's recorded start (count pass, scan, emit pass); a damaged image takes the serial
+ * reference-semantics walk (the one that re-decodes it), and so does every image when the environment variable
+ * JSGPU_DETAIL_WALK=1 is set (read once per process) or the MCU file map is off (want_mcu_map = 0).  Both give the same events.
+ * The context keeps the events and matrices of the last jsgpu_batch_decode (sized for them at each decode) until the next one;
+ * jsgpu_batch_detail_info / _events / _matrices read them in full, jsgpu_batch_detail returns the first JSGPU_MAX_DETAIL_*.
+ * In DC-only mode the printed MCUs are decoded in full (AC + IDCT), as DecodeScanCompPrint does. */
 typedef struct { int32_t enable; uint32_t image, mcu_x, mcu_y, len; } jsgpu_detail;
 #define JSGPU_DT_MCU    1   /* an MCU of the range starts: the blank separator line (ImgDecode.cpp:3249-3251)                     */
 #define JSGPU_DT_BLOCK  2   /* "    Lum (Tbl #0), MCU=[x,y]": a = DQT table, b = MCU x, c = MCU y (:1873-1889)                     */
@@ -320,12 +324,23 @@ typedef struct { uint32_t kind, seq, a, b, c, d, e, f; } jsgpu_detail_event;   /
 #define JSGPU_MAX_DETAIL_EVENTS 8192
 #define JSGPU_MAX_DETAIL_BLOCKS 512
 typedef struct {
-    uint32_t nevents, nblocks, pad0, pad1;       /* counted in full; the arrays keep the first JSGPU_MAX_DETAIL_* */
+    uint32_t nevents, nblocks, pad0, pad1;       /* counted in full; the arrays keep the first JSGPU_MAX_DETAIL_* (all of
+                                                    them: jsgpu_batch_detail_events / _matrices) */
     jsgpu_detail_event ev[JSGPU_MAX_DETAIL_EVENTS];
     int16_t matrix[JSGPU_MAX_DETAIL_BLOCKS][64]; /* m_anDctBlock: dequantised, natural order, [0] = the DC difference */
 } jsgpu_detail_dump;
 int jsgpu_set_detail(jsgpu_ctx* ctx, const jsgpu_detail* d);
 int jsgpu_batch_detail(jsgpu_ctx* ctx, jsgpu_detail_dump* out);
+/* info[0] = events, info[1] = blocks (matrices) of the last decode's detailed decode, in full; info[2] = the path that made them
+ * (JSGPU_DETAIL_SERIAL / JSGPU_DETAIL_PARALLEL); info[3] = 0.  Forces a sync. */
+#define JSGPU_DETAIL_SERIAL   0
+#define JSGPU_DETAIL_PARALLEL 1
+int jsgpu_batch_detail_info(jsgpu_ctx* ctx, uint32_t info[4]);
+/* Events first .. first+n-1 (n * 32 bytes), matrices first .. first+n-1 (n * 64 int16, natural order, [0] = the DC difference)
+ * of the last decode's detailed decode; JSGPU_EINVAL past info[0] / info[1].  A JSGPU_DT_MATRIX event's `a` indexes the
+ * matrices.  Force a sync. */
+int jsgpu_batch_detail_events(jsgpu_ctx* ctx, uint32_t first, uint32_t n, jsgpu_detail_event* out);
+int jsgpu_batch_detail_matrices(jsgpu_ctx* ctx, uint32_t first, uint32_t n, int16_t* out);
 
 /* --- Export-to-TIFF consumer (SURVEY.md §8f N4) ---------------------------------------------------------------------------
  * The three-samples-per-pixel, top-down array CJPEGsnoopDoc::OnToolsExporttiff (JPEGsnoopDoc.cpp:2061-2180) hands to

@@ -84,6 +84,15 @@ class jsgpu_colour_stats(C.Structure):
                 ("detail_rgb", (C.c_uint32 * 32) * 32)]
 
 
+class jsgpu_detail(C.Structure):
+    _fields_ = [("enable", C.c_int32), ("image", C.c_uint32), ("mcu_x", C.c_uint32), ("mcu_y", C.c_uint32), ("len", C.c_uint32)]
+
+
+# jsgpu_detail_event as a numpy record (kind JSGPU_DT_*, seq, a..f: include/jsgpu.h)
+DETAIL_EVENT_FIELDS = ("kind", "seq", "a", "b", "c", "d", "e", "f")
+DT_MCU, DT_BLOCK, DT_VLC, DT_MATRIX = 1, 2, 3, 4
+DETAIL_SERIAL, DETAIL_PARALLEL = 0, 1
+
 OUT_PIX_Y, OUT_PIX_CB, OUT_PIX_CR, OUT_DIB, OUT_BLK_Y, OUT_BLK_CB, OUT_BLK_CR, OUT_MCU_MAP, OUT_HISTO, OUT_STATS = range(10)
 
 # every symbol include/jsgpu.h and include/jsimg.h declare (tests check they are all exported)
@@ -92,7 +101,8 @@ JSGPU_SYMBOLS = [
     "jsgpu_set_idct_tables", "jsgpu_set_options", "jsgpu_get_options", "jsgpu_upload_tables", "jsgpu_bcast_tables",
     "jsgpu_batch_begin", "jsgpu_batch_layout", "jsgpu_batch_pools", "jsgpu_batch_upload", "jsgpu_batch_decode",
     "jsgpu_batch_download", "jsgpu_batch_stage_ms", "jsgpu_timer_start", "jsgpu_timer_stop", "jsgpu_batch_launches", "jsgpu_batch_selfsync_info", "jsgpu_batch_checksums", "jsgpu_batch_errors", "jsgpu_decode_batch_host",
-    "jsgpu_host_alloc", "jsgpu_host_free", "jsgpu_host_copy_rate", "jsgpu_set_preview", "jsgpu_batch_preview", "jsgpu_batch_colour_stats", "jsgpu_batch_export", "jsgpu_set_detail", "jsgpu_batch_detail"]
+    "jsgpu_host_alloc", "jsgpu_host_free", "jsgpu_host_copy_rate", "jsgpu_set_preview", "jsgpu_batch_preview", "jsgpu_batch_colour_stats", "jsgpu_batch_export", "jsgpu_set_detail", "jsgpu_batch_detail",
+    "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices"]
 JSIMG_SYMBOLS = [
     "jsimg_create", "jsimg_destroy", "jsimg_config", "jsimg_set_file", "jsimg_overlay_install", "jsimg_overlay_remove_all", "jsimg_Reset", "jsimg_ResetState",
     "jsimg_SetDqtEntry", "jsimg_SetDqtTables", "jsimg_GetDqtEntry", "jsimg_SetDhtTables", "jsimg_SetDhtEntry",
@@ -153,6 +163,9 @@ def load():
     L.jsimg_tiff_write.argtypes = [C.c_char_p, i32, i32, vp, u32, u32]
     L.jsgpu_set_detail.argtypes = [vp, vp]
     L.jsgpu_batch_detail.argtypes = [vp, vp]
+    L.jsgpu_batch_detail_info.argtypes = [vp, vp]
+    L.jsgpu_batch_detail_events.argtypes = [vp, u32, u32, vp]
+    L.jsgpu_batch_detail_matrices.argtypes = [vp, u32, u32, vp]
     L.jsimg_SetDetailVlc.argtypes = [vp, i32, u32, u32, u32]; L.jsimg_SetDetailVlc.restype = None
     L.jsimg_GetDetailVlc.argtypes = [vp] + [C.POINTER(u32)] * 4; L.jsimg_GetDetailVlc.restype = None
     L.jsimg_config_histo.argtypes = [vp, i32, i32, i32]; L.jsimg_config_histo.restype = None

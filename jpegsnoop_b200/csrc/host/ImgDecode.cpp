@@ -416,20 +416,35 @@ void CimgDecode::DecodeScanImg(unsigned nStart, bool bDisplay, bool bQuiet)
     bool bMarkerNoteLogged = false;
     {
         jsgpu_scan_errors* pErr = new jsgpu_scan_errors; memset(pErr, 0, 16);
-        jsgpu_detail_dump* pDet = m_bDetailVlc ? new jsgpu_detail_dump : nullptr;
+        uint32_t anDetInfo[4] = { 0, 0, 0, 0 };
         const bool bExact = (lo.status & JSGPU_ST_EXACT) != 0;
-        const bool bHaveDet = pDet && jsgpu_batch_detail(m_pGpu, pDet) == JSGPU_OK;
+        const bool bHaveDet = m_bDetailVlc && jsgpu_batch_detail_info(m_pGpu, anDetInfo) == JSGPU_OK;
         const bool bHaveErr = (bExact || bHaveDet) && jsgpu_batch_errors(m_pGpu, 0, pErr) == JSGPU_OK;
         const unsigned nEv = bHaveErr ? (pErr->nevents < JSGPU_MAX_EVENTS ? pErr->nevents : JSGPU_MAX_EVENTS) : 0;
         unsigned iEv = 0;
         if (bHaveDet) {
-            const unsigned nDet = pDet->nevents < JSGPU_MAX_DETAIL_EVENTS ? pDet->nevents : JSGPU_MAX_DETAIL_EVENTS;
-            for (unsigned i = 0; i < nDet; i++) {
-                for (; iEv < nEv && iEv < pDet->ev[i].seq; iEv++) { if (pErr->ev[iEv].code == JSGPU_EV_MARKER_NOTE) bMarkerNoteLogged = true; LogScanEvent(pErr->ev[iEv]); }
-                LogDetailEvent(pDet->ev[i], *pDet);
+            // every event and matrix, read in pages (the matrices in the order the events name them)
+            const unsigned nDet = anDetInfo[0], nBlk = anDetInfo[1], nPage = 4096, nMatPage = 512;
+            std::vector<jsgpu_detail_event> vEv(nPage);
+            std::vector<int16_t> vMat((size_t)nMatPage * 64);
+            unsigned nMatFirst = 0, nMatHave = 0;
+            for (unsigned nFirst = 0; nFirst < nDet; nFirst += nPage) {
+                const unsigned n = (nDet - nFirst < nPage) ? nDet - nFirst : nPage;
+                if (jsgpu_batch_detail_events(m_pGpu, nFirst, n, vEv.data()) != JSGPU_OK) break;
+                for (unsigned i = 0; i < n; i++) {
+                    const jsgpu_detail_event& e = vEv[i];
+                    for (; iEv < nEv && iEv < e.seq; iEv++) { if (pErr->ev[iEv].code == JSGPU_EV_MARKER_NOTE) bMarkerNoteLogged = true; LogScanEvent(pErr->ev[iEv]); }
+                    const int16_t* pMat = nullptr;
+                    if (e.kind == JSGPU_DT_MATRIX && e.a < nBlk) {
+                        if (e.a < nMatFirst || e.a >= nMatFirst + nMatHave) {
+                            nMatFirst = e.a; nMatHave = (nBlk - e.a < nMatPage) ? nBlk - e.a : nMatPage;
+                            if (jsgpu_batch_detail_matrices(m_pGpu, nMatFirst, nMatHave, vMat.data()) != JSGPU_OK) nMatHave = 0;
+                        }
+                        if (e.a >= nMatFirst && e.a < nMatFirst + nMatHave) pMat = &vMat[(size_t)(e.a - nMatFirst) * 64];
+                    }
+                    LogDetailEvent(e, pMat);
+                }
             }
-            if (pDet->nevents > JSGPU_MAX_DETAIL_EVENTS)
-                m_pLog->AddLineWarn(JS_LOGSTR(fmt("    (%u further detailed-decode lines not itemised)", pDet->nevents - JSGPU_MAX_DETAIL_EVENTS)));
         }
         if (bExact) {
             if (bHaveErr) {
@@ -448,7 +463,7 @@ void CimgDecode::DecodeScanImg(unsigned nStart, bool bDisplay, bool bQuiet)
             for (; iEv < nEv; iEv++) { if (pErr->ev[iEv].code == JSGPU_EV_MARKER_NOTE) bMarkerNoteLogged = true; LogScanEvent(pErr->ev[iEv]); }
             if (lo.status) { m_bScanBad = true; m_pLog->AddLineErr(JS_LOGSTR(fmt("*** ERROR: Bad scan data (device status 0x%08X) ***", lo.status))); }
         }
-        delete pErr; delete pDet;
+        delete pErr;
     }
     if (!(lo.status & JSGPU_ST_EXACT)) {
         // A healthy scan still leaves one line behind: topping the accumulator up past the last data byte meets the marker
@@ -544,7 +559,7 @@ void CimgDecode::LogScanEvent(const jsgpu_scan_event& e)
 void CimgDecode::SetDetailVlc(bool bDetail, unsigned nX, unsigned nY, unsigned nLen) { m_bDetailVlc = bDetail; m_nDetailVlcX = nX; m_nDetailVlcY = nY; m_nDetailVlcLen = nLen; }
 void CimgDecode::GetDetailVlc(bool& bDetail, unsigned& nX, unsigned& nY, unsigned& nLen) { bDetail = m_bDetailVlc; nX = m_nDetailVlcX; nY = m_nDetailVlcY; nLen = m_nDetailVlcLen; }
 
-void CimgDecode::LogDetailEvent(const jsgpu_detail_event& e, const jsgpu_detail_dump& d)
+void CimgDecode::LogDetailEvent(const jsgpu_detail_event& e, const int16_t* pMatrix)
 {
     switch (e.kind) {
     case JSGPU_DT_MCU: m_pLog->AddLine(JS_LOGSTR("")); break;                                          // ref :3249-3251
@@ -578,10 +593,10 @@ void CimgDecode::LogDetailEvent(const jsgpu_detail_event& e, const jsgpu_detail_
             m_pLog->AddLine(JS_LOGSTR(fmt("      [0x%08X.%u]: ZRL=[%2u] Val=[%5d] Coef=[%02u..%02u] Data=[%s] %s", nVlcPos, nVlcAlign, nZrl, nVal, nCoeffStart, nCoeffEnd, strData.c_str(), kSpecial[e.f & 3])));
         break; }
     case JSGPU_DT_MATRIX: {                                                                            // ReportDctMatrix, ref :2104-2131
-        if (e.a >= JSGPU_MAX_DETAIL_BLOCKS) break;
+        if (!pMatrix) break;
         for (unsigned nY = 0; nY < 8; nY++) {
             std::string strLine = nY == 0 ? "                      DCT Matrix=[" : "                                 [";
-            for (unsigned nX = 0; nX < 8; nX++) { strLine += fmt("%5d", (int)d.matrix[e.a][nY * 8 + nX]); if (nX != 7) strLine += " "; }
+            for (unsigned nX = 0; nX < 8; nX++) { strLine += fmt("%5d", (int)pMatrix[nY * 8 + nX]); if (nX != 7) strLine += " "; }
             strLine += "]";
             m_pLog->AddLine(JS_LOGSTR(strLine));
         }

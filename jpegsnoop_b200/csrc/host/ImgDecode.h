@@ -186,7 +186,7 @@ private:
     void        PreviewSettings(jsgpu_preview& pv) const;
     void        FetchPreviewResults();
     void        LogScanEvent(const jsgpu_scan_event& e);          // one error event of a damaged scan -> the reference's line(s)
-    void        LogDetailEvent(const jsgpu_detail_event& e, const jsgpu_detail_dump& d);   // ReportVlc / ReportDctMatrix lines
+    void        LogDetailEvent(const jsgpu_detail_event& e, const int16_t* pMatrix);   // ReportVlc / ReportDctMatrix lines (pMatrix: 64 entries, for JSGPU_DT_MATRIX)
     void        LogYccNote(const jsgpu_ycc_warn& w);
     void        LogDetailRgb(const jsgpu_colour_stats* cs);       // "Detailed IDCT Dump (RGB)" of CalcChannelPreviewFull, with the YCC notes in between            // DIB, average luminance, statistics and "YCC Clipped" notes of the last preview pass
 

@@ -71,7 +71,11 @@ struct jsgpu_ctx {
     DevBuf d_mc; uint32_t mc_total = 0;      // marker-scan chunk arrays
     DevBuf d_cstats, d_rowclip; uint64_t rows_total = 0; uint32_t max_hp = 0; bool pv_done = false;
     // "Detailed Decode" request (jsgpu_set_detail) and the dump of the last decode
-    jsgpu_detail dtl = {0, 0, 0, 0, 0}; DevBuf d_detail; bool dt_done = false;
+    jsgpu_detail dtl = {0, 0, 0, 0, 0}; bool dt_done = false;
+    DevBuf d_dt_ev, d_dt_mat;                // events and matrices, sized at each decode
+    DevBuf d_dt_scratch;                     // [16] counters (JsDetailOut::hdr), [136] the walk's code-length histogram, then the
+                                             // parallel path's per-MCU event counts / offsets and last top-up points
+    bool dt_parallel = false; JsDetailRange dt_range = {0, 0, 0, 0, 0}; JsDetailOut dt_out = {};
 };
 
 static int fail(jsgpu_ctx* c, int code, const char* fmt, ...)
@@ -150,7 +154,7 @@ void jsgpu_free(jsgpu_ctx* ctx)
     ctx->kids.clear();
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    DevBuf* bufs[] = { &ctx->d_ctab, &ctx->d_li, &ctx->d_lf, &ctx->d_sym, &ctx->d_tables, &ctx->d_img, &ctx->d_items, &ctx->d_litems, &ctx->d_tiles, &ctx->d_ubits, &ctx->d_seg64, &ctx->d_ph, &ctx->d_rowtab, &ctx->d_ex, &ctx->d_cstats, &ctx->d_rowclip, &ctx->d_detail, &ctx->d_mc, &ctx->d_bits, &ctx->d_seg,
+    DevBuf* bufs[] = { &ctx->d_ctab, &ctx->d_li, &ctx->d_lf, &ctx->d_sym, &ctx->d_tables, &ctx->d_img, &ctx->d_items, &ctx->d_litems, &ctx->d_tiles, &ctx->d_ubits, &ctx->d_seg64, &ctx->d_ph, &ctx->d_rowtab, &ctx->d_ex, &ctx->d_cstats, &ctx->d_rowclip, &ctx->d_dt_ev, &ctx->d_dt_mat, &ctx->d_dt_scratch, &ctx->d_mc, &ctx->d_bits, &ctx->d_seg,
                        &ctx->d_coef, &ctx->d_mcubits, &ctx->d_pix, &ctx->d_dib, &ctx->d_blk, &ctx->d_mcumap, &ctx->d_histo, &ctx->d_stats, &ctx->d_misc };
     for (auto* b : bufs) b->release();
     for (auto& ev : ctx->ev) if (ev) cudaEventDestroy(ev);
@@ -593,6 +597,53 @@ static int host_marker_walk(jsgpu_ctx* ctx, const uint8_t* bits_host)
     return 0;
 }
 
+// The detailed decode of this batch's image ctx->dtl.image (jsgpu_set_detail): picks the path and sizes the event and matrix
+// arrays.  A healthy image (status 0 after the Huffman stage: one sync) is decoded one thread per MCU; the count pass and scan
+// run now (a second sync reads the totals, so the arrays are sized exactly), the emit pass after the MCU file map.  Otherwise
+// the serial walk fills arrays sized for the most it can report: 1 + 66 events per block (a separator per MCU; per block a
+// heading, at most 64 symbols, a matrix) and one matrix per block, for the printed MCUs.
+static int detail_prepare(jsgpu_ctx* ctx, int err_max, int* launches)
+{
+    static const bool force_walk = [] { const char* e = getenv("JSGPU_DETAIL_WALK"); return e && atoi(e) == 1; }();
+    const DevBatch& b = ctx->batch;
+    cudaStream_t s = ctx->stream;
+    const jsgpu_detail& dtl = ctx->dtl;
+    const DevImage& im = ctx->himg[dtl.image];
+    // the walk decodes MCUs 0 .. end-1 and prints those from base on (its arithmetic: a 32-bit base, a 64-bit end)
+    const uint32_t base = dtl.mcu_y * im.mcu_xmax + dtl.mcu_x;
+    const uint32_t end = im.valid ? (uint32_t)std::min<unsigned long long>(im.nmcu, (unsigned long long)base + dtl.len) : 0u;
+    JsDetailRange r;
+    r.image = dtl.image; r.base = base; r.nprint = (base < end) ? end - base : 0u;
+    r.first = (base < end) ? (base ? base - 1 : 0u) : (end ? end - 1 : 0u);
+    r.n = end ? end - r.first : 0u;
+    uint32_t status = 1;
+    if (im.valid && !force_walk && ctx->opt.want_mcu_map) {
+        CK(cudaMemcpyAsync(&status, b.img_status + dtl.image, 4, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+    }
+    CK(ctx->d_dt_scratch.reserve((16 + 136 + 2 * (size_t)r.n) * 4));
+    uint32_t* hdr = (uint32_t*)ctx->d_dt_scratch.p;
+    CK(cudaMemsetAsync(hdr, 0, 16 * 4, s));
+    uint64_t nev, nmat;
+    if (status == 0) {
+        *launches += js_launch_detail_count(b, r, hdr + 16 + 136, hdr, err_max, s);
+        uint32_t tot[2];
+        CK(cudaMemcpyAsync(tot, hdr, sizeof tot, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        nev = tot[0]; nmat = tot[1];
+    } else {
+        nev = (uint64_t)r.nprint * (1 + (uint64_t)im.bpm * 66);
+        nmat = (uint64_t)r.nprint * im.bpm;
+    }
+    CK(ctx->d_dt_ev.reserve(std::max<uint64_t>(nev, 1) * sizeof(jsgpu_detail_event)));
+    CK(ctx->d_dt_mat.reserve(std::max<uint64_t>(nmat, 1) * 64 * sizeof(int16_t)));
+    ctx->dt_out.ev = (jsgpu_detail_event*)ctx->d_dt_ev.p; ctx->dt_out.mat = (int16_t*)ctx->d_dt_mat.p; ctx->dt_out.hdr = hdr;
+    ctx->dt_out.ev_cap = nev; ctx->dt_out.mat_cap = nmat;
+    ctx->dt_range = r;
+    ctx->dt_parallel = status == 0;
+    return JSGPU_OK;
+}
+
 int jsgpu_batch_decode(jsgpu_ctx* ctx)
 {
     if (!ctx) return JSGPU_EINVAL;
@@ -652,17 +703,19 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx)
             launches += js_launch_selfsync(bh, ctx->sm_count, s);
             launches += js_launch_huffman_lane_vseg(bh, ctx->sm_count, s);
         }
-        // damaged images (status word != 0) are decoded again with the reference's semantics; returns at once for the others
-        ctx->dt_done = false;
+        // the detailed decode of a healthy image: count pass and scan here, events after the MCU file map (below)
+        const int err_max = ctx->opt.scan_err_max > 0 ? ctx->opt.scan_err_max : 20;
+        ctx->dt_done = ctx->dt_parallel = false;
         jsgpu_detail dtl = ctx->dtl;
         if (dtl.enable && dtl.image < b.nimg) {
-            CK(ctx->d_detail.reserve(sizeof(jsgpu_detail_dump) + 2 * 4 * 17 * 4));
-            CK(cudaMemsetAsync(ctx->d_detail.p, 0, 16, s));
+            int rc = detail_prepare(ctx, err_max, &launches);
+            if (rc != JSGPU_OK) return rc;
             ctx->dt_done = true;
+            if (ctx->dt_parallel) dtl.enable = 0;
         } else dtl.enable = 0;
-        jsgpu_detail_dump* dump = (jsgpu_detail_dump*)ctx->d_detail.p;
-        launches += js_launch_exact(b, ctx->opt.scan_err_max > 0 ? ctx->opt.scan_err_max : 20, dtl, dump,
-                                    dump ? (uint32_t*)((uint8_t*)dump + sizeof(jsgpu_detail_dump)) : nullptr, s);
+        // damaged images (status word != 0) are decoded again with the reference's semantics (and the detail image, when it takes
+        // the serial walk); returns at once for the others
+        launches += js_launch_exact(b, err_max, dtl, ctx->dt_out, ctx->dt_done ? (uint32_t*)ctx->d_dt_scratch.p + 16 : nullptr, s);
     }
     // The MCU file map depends on the Huffman stage only: its kernels run on a second stream while the IDCT kernel has the device
     // (they are short and latency-bound); the scalar statistics below wait for both.
@@ -672,6 +725,7 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx)
         CK(cudaStreamWaitEvent(ctx->stream2, ctx->evx[0], 0));
         launches += js_launch_finalize_maps(b, ctx->stream2);
         launches += js_launch_finalize_emptied(b, ctx->stream2);
+        if (ctx->dt_parallel) launches += js_launch_detail_emit(b, ctx->dt_range, (const uint32_t*)ctx->d_dt_scratch.p + 16 + 136, ctx->dt_out, ctx->stream2);
         CK(cudaEventRecord(ctx->evx[1], ctx->stream2));
         maps_forked = true;
     }
@@ -737,14 +791,54 @@ int jsgpu_set_detail(jsgpu_ctx* ctx, const jsgpu_detail* d)
     return JSGPU_OK;
 }
 
+int jsgpu_batch_detail_info(jsgpu_ctx* ctx, uint32_t info[4])
+{
+    if (!ctx || !info) return JSGPU_EINVAL;
+    if (!ctx->decoded || ctx->host_delivered || !ctx->dt_done) return fail(ctx, JSGPU_ESTATE, "the last decode collected no detailed decode (jsgpu_set_detail)");
+    cudaSetDevice(ctx->device);
+    CK(cudaMemcpyAsync(info, ctx->dt_out.hdr, 2 * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    info[2] = ctx->dt_parallel ? JSGPU_DETAIL_PARALLEL : JSGPU_DETAIL_SERIAL; info[3] = 0;
+    return JSGPU_OK;
+}
+
+int jsgpu_batch_detail_events(jsgpu_ctx* ctx, uint32_t first, uint32_t n, jsgpu_detail_event* out)
+{
+    if (!ctx || (!out && n)) return JSGPU_EINVAL;
+    uint32_t info[4];
+    int rc = jsgpu_batch_detail_info(ctx, info);
+    if (rc != JSGPU_OK) return rc;
+    if ((uint64_t)first + n > std::min<uint64_t>(info[0], ctx->dt_out.ev_cap))
+        return fail(ctx, JSGPU_EINVAL, "events %u..%llu asked, the detailed decode has %u", first, (unsigned long long)first + n, info[0]);
+    if (n) CK(cudaMemcpyAsync(out, ctx->dt_out.ev + first, (size_t)n * sizeof *out, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return JSGPU_OK;
+}
+
+int jsgpu_batch_detail_matrices(jsgpu_ctx* ctx, uint32_t first, uint32_t n, int16_t* out)
+{
+    if (!ctx || (!out && n)) return JSGPU_EINVAL;
+    uint32_t info[4];
+    int rc = jsgpu_batch_detail_info(ctx, info);
+    if (rc != JSGPU_OK) return rc;
+    if ((uint64_t)first + n > std::min<uint64_t>(info[1], ctx->dt_out.mat_cap))
+        return fail(ctx, JSGPU_EINVAL, "matrices %u..%llu asked, the detailed decode has %u", first, (unsigned long long)first + n, info[1]);
+    if (n) CK(cudaMemcpyAsync(out, ctx->dt_out.mat + (size_t)first * 64, (size_t)n * 64 * sizeof *out, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return JSGPU_OK;
+}
+
 int jsgpu_batch_detail(jsgpu_ctx* ctx, jsgpu_detail_dump* out)
 {
     if (!ctx || !out) return JSGPU_EINVAL;
-    if (!ctx->decoded || ctx->host_delivered || !ctx->dt_done) return fail(ctx, JSGPU_ESTATE, "the last decode collected no detailed decode (jsgpu_set_detail)");
-    cudaSetDevice(ctx->device);
-    CK(cudaMemcpyAsync(out, ctx->d_detail.p, sizeof *out, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    return JSGPU_OK;
+    uint32_t info[4];
+    int rc = jsgpu_batch_detail_info(ctx, info);
+    if (rc != JSGPU_OK) return rc;
+    memset(out, 0, sizeof *out);
+    out->nevents = info[0]; out->nblocks = info[1];
+    rc = jsgpu_batch_detail_events(ctx, 0, std::min<uint32_t>(info[0], JSGPU_MAX_DETAIL_EVENTS), out->ev);
+    if (rc == JSGPU_OK) rc = jsgpu_batch_detail_matrices(ctx, 0, std::min<uint32_t>(info[1], JSGPU_MAX_DETAIL_BLOCKS), &out->matrix[0][0]);
+    return rc;
 }
 
 int jsgpu_batch_export(jsgpu_ctx* ctx, uint32_t image, int mode, void* host_out, uint64_t bytes)

@@ -182,7 +182,17 @@ int js_launch_idct_fused(const DevBatch& b, const IdctSym* sym, const ColorTabs*
 int js_idct_baked_matches(const int32_t* li);
 int js_idctf_baked_matches(const float* lf);
 int js_launch_build_color_tables(ColorTabs* t, cudaStream_t s);
-int js_launch_exact(const DevBatch& b, int err_max, const jsgpu_detail& dtl, jsgpu_detail_dump* dump, uint32_t* scratch_histo, cudaStream_t s);       // damaged images, again, with the reference's semantics (jsgpu_exact.cu)
+// "Detailed Decode" (jsgpu_set_detail): where it writes — the event and matrix arrays the context sized for this decode and
+// their counters (hdr[0] events, hdr[1] blocks, counted in full; an array keeps what fits its capacity; hdr[2] the path) ...
+struct JsDetailOut {
+    jsgpu_detail_event* ev; int16_t* mat; uint32_t* hdr;
+    unsigned long long ev_cap, mat_cap;
+};
+// ... and, for the parallel path (jsgpu_detail.cu), which MCUs: first .. first+n-1 are decoded, base .. base+nprint-1 printed
+struct JsDetailRange { uint32_t image, base, first, n, nprint; };
+int js_launch_exact(const DevBatch& b, int err_max, const jsgpu_detail& dtl, const JsDetailOut& dump, uint32_t* scratch_histo, cudaStream_t s);       // damaged images, again, with the reference's semantics (jsgpu_exact.cu)
+int js_launch_detail_count(const DevBatch& b, const JsDetailRange& r, uint32_t* scratch, uint32_t* hdr, int err_max, cudaStream_t s);   // count pass + scan (+ DC-only rows)
+int js_launch_detail_emit(const DevBatch& b, const JsDetailRange& r, const uint32_t* scratch, const JsDetailOut& out, cudaStream_t s);  // events + matrices (after the MCU file map)
 int js_launch_export(const DevBatch& b, uint32_t image, int mode, uint8_t* out, uint64_t npx, int sm_count, cudaStream_t s);   // Export-to-TIFF sample array
 int js_launch_finalize_maps(const DevBatch& b, cudaStream_t s);     // MCU file map (independent of the IDCT)
 int js_launch_finalize_stats(const DevBatch& b, cudaStream_t s);    // brightest pixel / average luma / end-of-scan position (after the IDCT)

@@ -15,6 +15,7 @@
 // colour math uses __fmul_rn/__fadd_rn/__fsub_rn/__fdiv_rn so no FMA contraction can happen.
 #include "jsgpu_internal.h"
 #include "jsgpu_ycc.cuh"
+#include "jsgpu_detail.cuh"     // js_raw_of_unstuffed
 #include <cstdio>
 #include <cstdlib>
 #include <algorithm>
@@ -382,7 +383,6 @@ int js_launch_idct_simple(const DevBatch& b, const int32_t* li, const float* lf,
 // K3: finalisation — scalar statistics (ImgDecode.cpp:4802-4819) and the MCU file map.  (The block-DC maps,
 // :3524-3608, are written by the Huffman kernels.)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t js_raw_of_unstuffed(const DevBatch& b, const DevImage& im, uint32_t k, uint32_t u);
 __global__ void k_finalize_stats(DevBatch b)
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -473,42 +473,6 @@ __global__ void __launch_bounds__(128) k_finalize_mcumap(DevBatch b)
         tcur++;
     }
     }
-}
-
-// Raw offset (inside interval k of image im) of unstuffed byte u: u plus the stuffed zeros before it — from the short list
-// k_unstuff keeps per interval, from the row table of k_unstuff_long (long intervals), or, for a short interval with more
-// stuffed bytes than the list holds, by walking its raw bytes.
-__device__ __forceinline__ uint32_t js_raw_of_unstuffed(const DevBatch& b, const DevImage& im, uint32_t k, uint32_t u)
-{
-    const uint32_t sidx = im.seg_first + k, ns = b.seg_nstuff[sidx];
-    const uint32_t s0 = b.seg_start[sidx], len = b.seg_end[sidx] - s0;
-    if (im.psync) {
-        const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(b.bits + im.scan_off + s0) & 3);
-        const size_t rt0 = (size_t)(im.rt_off + (s0 >> 7) + 2u * k);
-        const uint32_t nrows = (len + mis + 127) >> 7;
-        uint32_t lo = u >> 7, hi = min(nrows - 1, (u + ns + mis) >> 7);      // rowtab[r] <= 128 r: the row holding u is not before u / 128
-        while (lo < hi) { const uint32_t mid = (lo + hi + 1) >> 1; if (b.rowtab[rt0 + mid] <= u) lo = mid; else hi = mid - 1; }
-        uint32_t need = u - b.rowtab[rt0 + lo];                     // kept bytes of the row before the one we want
-        const uint4 mk = b.rowmask[rt0 + lo];
-        uint32_t w = ~mk.x, off = 0, c = __popc(w);                  // set bit = this raw byte of the row is kept
-        if (need >= c) { need -= c; w = ~mk.y; off = 32; c = __popc(w);
-            if (need >= c) { need -= c; w = ~mk.z; off = 64; c = __popc(w);
-                if (need >= c) { need -= c; w = ~mk.w; off = 96; } } }
-        return (lo << 7) - mis + off + __fns(w, 0, (int)need + 1);
-    }
-    if (ns <= JS_STUFF_LIST) {
-        uint32_t raw = u;
-        for (uint32_t j = 0; j < ns; j++) raw += (b.seg_stuff[(size_t)sidx * JS_STUFF_LIST + j] < u) ? 1u : 0u;
-        return raw;
-    }
-    const uint8_t* seg = b.bits + im.scan_off + s0;
-    uint32_t r = 0, kept = 0;
-    for (; r < len; r++) {
-        if (seg[r] == 0 && r > 0 && seg[r - 1] == 0xFF) continue;
-        if (kept == u) break;
-        kept++;
-    }
-    return r;
 }
 
 // Fast MCU file map: one thread per MCU, using the stuffed-byte list k_unstuff recorded per interval

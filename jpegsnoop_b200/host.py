@@ -317,6 +317,25 @@ class BatchDecoder:
         a = np.zeros(16, np.uint32); self._ck(self.L.jsgpu_batch_selfsync_info(self.ctx, a.ctypes.data, 16))
         return int(a[0]), int(a[1]), [int(v) for v in a[3:3 + int(a[2])]]
 
+    def set_detail(self, image, x=0, y=0, n=1, enable=True):
+        """jsgpu_set_detail: the next decode also reports the "Detailed Decode" of `n` MCUs of image `image` from MCU (x, y)."""
+        d = B.jsgpu_detail(enable=int(enable), image=image, mcu_x=x, mcu_y=y, len=n)
+        self._ck(self.L.jsgpu_set_detail(self.ctx, C.byref(d)))
+
+    def detail_info(self):
+        """(events, blocks, path) of the last decode's detailed decode; path is B.DETAIL_SERIAL or B.DETAIL_PARALLEL."""
+        a = np.zeros(4, np.uint32); self._ck(self.L.jsgpu_batch_detail_info(self.ctx, a.ctypes.data))
+        return int(a[0]), int(a[1]), int(a[2])
+
+    def detail(self):
+        """The last decode's detailed decode in full: (events uint32 [n, 8] — columns B.DETAIL_EVENT_FIELDS, kind JSGPU_DT_* —,
+        matrices int16 [blocks, 64], natural order, [0] = the DC difference)."""
+        nev, nblk, _ = self.detail_info()
+        ev = np.zeros((nev, 8), np.uint32); mat = np.zeros((nblk, 64), np.int16)
+        self._ck(self.L.jsgpu_batch_detail_events(self.ctx, 0, nev, ev.ctypes.data))
+        self._ck(self.L.jsgpu_batch_detail_matrices(self.ctx, 0, nblk, mat.ctypes.data))
+        return ev, mat
+
     def timer_start(self): self._ck(self.L.jsgpu_timer_start(self.ctx))
 
     def timer_stop(self):
