@@ -102,7 +102,7 @@ typedef struct {
                                kernel where it applies, simple kernels elsewhere                   */
     int32_t want_histo;     /* accumulate m_anDhtHisto (ImgDecode.cpp:1190-1191); default 1      */
     int32_t want_mcu_map;   /* build m_pMcuFileMap (ImgDecode.cpp:3229); default 1               */
-    int32_t device_markers; /* 1 = find RSTn/end-of-scan on the GPU (default), 0 = host walk      */
+    int32_t device_markers; /* ignored: RSTn and the end of scan are always found on the GPU      */
     int32_t scan_err_max;   /* CSnoopConfig::nErrMaxDecodeScan (SnoopConfig.cpp:89): capped error lines
                                per scan; 0 = the reference's default, 20                          */
 } jsgpu_options;

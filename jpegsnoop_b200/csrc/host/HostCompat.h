@@ -82,5 +82,4 @@ struct CSnoopConfig {
     int      nCudaDevice = 0;
     int      nHuffKernel = 0;             // jsgpu_options.huff_kernel
     int      nIdctKernel = 0;             // jsgpu_options.idct_kernel
-    bool     bDeviceMarkers = true;
 };

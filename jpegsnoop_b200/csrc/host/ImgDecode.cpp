@@ -31,7 +31,6 @@ static const bool kCfgIdctFixed = false;
 #define JS_CFG_DEVICE(c)       0
 #define JS_CFG_HUFF(c)         0
 #define JS_CFG_IDCTK(c)        0
-#define JS_CFG_DEVMARKERS(c)   true
 #else
 #define JS_LOGSTR(x) std::string(x)
 static void js_copy_scan(CwindowBuf* w, unsigned long off, size_t n, uint8_t* dst) { w->BufCopy(off, n, dst); }
@@ -39,7 +38,6 @@ static void js_copy_scan(CwindowBuf* w, unsigned long off, size_t n, uint8_t* ds
 #define JS_CFG_DEVICE(c)       ((c)->nCudaDevice)
 #define JS_CFG_HUFF(c)         ((c)->nHuffKernel)
 #define JS_CFG_IDCTK(c)        ((c)->nIdctKernel)
-#define JS_CFG_DEVMARKERS(c)   ((c)->bDeviceMarkers)
 #endif
 
 CimgDecode::CimgDecode(CDocLog* pLog, CwindowBuf* pWBuf, CSnoopConfig* pConfig)
@@ -345,7 +343,6 @@ void CimgDecode::DecodeScanImg(unsigned nStart, bool bDisplay, bool bQuiet)
     opt.idct_mode = JS_CFG_IDCT_FIXED(m_pAppConfig) ? 0 : 1;
     opt.decode_ac = m_bDecodeScanAc ? 1 : 0;
     opt.huff_kernel = JS_CFG_HUFF(m_pAppConfig); opt.idct_kernel = JS_CFG_IDCTK(m_pAppConfig);
-    opt.device_markers = JS_CFG_DEVMARKERS(m_pAppConfig) ? 1 : 0;
     opt.want_histo = 1; opt.want_mcu_map = 1;
     opt.scan_err_max = (int32_t)m_nScanErrMax;
     jsgpu_set_options(m_pGpu, &opt);

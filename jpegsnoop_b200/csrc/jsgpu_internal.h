@@ -52,7 +52,7 @@ struct DevTableSet {
 // Device descriptor of one image of the batch.
 struct DevImage {
     uint32_t valid;                 // 0 = skipped (the reference would return early)
-    uint32_t dim_x, dim_y, ns, precision;
+    uint32_t ns, precision;
     uint32_t mcu_w, mcu_h, mcu_xmax, mcu_ymax, blk_xmax, blk_ymax, wp, hp;
     uint32_t nmcu;
     uint32_t ri;                    // MCUs per restart interval (= nmcu when DRI is off)
@@ -74,9 +74,6 @@ struct DevImage {
     uint32_t std_layout;            // 1 = every component has H in {1,Hmax} and V in {1,Vmax} (fused IDCT kernel applies)
     uint32_t tile_mcus;             // MCUs per IDCT tile (32 / Hmax)
     uint32_t tiles_per_row;
-    uint32_t tile_groups;           // 32-block groups per IDCT tile
-    uint32_t item_first, nitems;    // Huffman work items (groups of HUFF_WARPS segments)
-    uint32_t tile_first, ntiles;    // IDCT tiles
     uint32_t psync;                 // 1 = long restart intervals: decoded through the self-synchronising passes (jsgpu_phuff_core.cuh)
     uint32_t ph_nslots;             // ... number of 4096-bit slots reserved for this image (its slot arrays hold ph_nslots + 1 entries)
     uint64_t ph_first;              // ... first entry of this image in the slot arrays
@@ -163,7 +160,6 @@ struct DevBatch {
 #define JS_LANE_SEGS  256            // restart intervals per CTA pass, lane kernel (8 warps x 32 lanes)
 #define JS_LANE_L2S   512            // second-level entries per table the lane kernel stages in shared memory
 #define JS_LANE_TAB   (JS_LUT_SIZE + JS_LANE_L2S)   // entries per staged table: first level, then its second level
-#define JS_ROWTAB_MIN 2048           // raw bytes from which an interval gets a row table
 #define JS_PSYNC_MIN_BLOCKS 192      // blocks per restart interval from which an image takes the self-synchronising path
 
 // launchers (jsgpu_kernels.cu) — each returns the number of kernels it enqueued

@@ -20,61 +20,39 @@
 #define PH_THREADS 256
 
 struct PhShared {
-    uint32_t qz[3][80];
-    uint32_t lslot[6], li[6];
-    uint32_t nl, bpm, pshift, pad;
+    LaneTabs t;
+    uint32_t bpm, pshift;
     uint16_t blk_dc[PH_MAX_BPM], blk_ac[PH_MAX_BPM];
     uint8_t  blk_c[PH_MAX_BPM];
 };
+static_assert(sizeof(PhShared) % 16 == 0, "the staged tables behind PhShared are read as uint4");
 
-// The image's MCU layout (thread 0): which staged table every block of an MCU decodes with, its component, the blocks per
-// MCU and the precision's divide.  It depends on the sampling factors and the precision, which (table_set, tab_sig) does not
-// capture: images that share their staged tables can still differ here.
+// The image's MCU layout (thread 0, after lane_stage): which staged table every block of an MCU decodes with, its component,
+// the blocks per MCU and the precision's divide.  It depends on the sampling factors and the precision, which (table_set,
+// tab_sig) does not capture: images that share their staged tables can still differ here.
 __device__ __forceinline__ void ph_layout(PhShared& sh, const DevImage& im)
 {
-    uint32_t n = 0;
-    for (uint32_t c = 0; c < im.ns; c++) for (uint32_t cls = 0; cls < 2; cls++) {
-        const uint32_t slot = cls ? im.slot_ac[c] : im.slot_dc[c];
-        uint32_t j = 0;
-        while (j < n && sh.lslot[j] != slot) j++;
-        if (j == n) sh.lslot[n++] = slot;
-        sh.li[c * 2 + cls] = j;
-    }
-    sh.nl = n;
     uint32_t bi = 0;
     for (uint32_t c = 0; c < im.ns; c++)
         for (uint32_t q = 0; q < im.H[c] * im.V[c] && bi < PH_MAX_BPM; q++, bi++) {
-            sh.blk_dc[bi] = (uint16_t)(sh.li[c * 2] * JS_LANE_TAB); sh.blk_ac[bi] = (uint16_t)(sh.li[c * 2 + 1] * JS_LANE_TAB); sh.blk_c[bi] = (uint8_t)c;
+            sh.blk_dc[bi] = (uint16_t)(sh.t.li[c * 2] * JS_LANE_TAB); sh.blk_ac[bi] = (uint16_t)(sh.t.li[c * 2 + 1] * JS_LANE_TAB); sh.blk_c[bi] = (uint8_t)c;
         }
     sh.bpm = bi;
     sh.pshift = (im.precision > 8) ? im.precision - 8 : 0;
 }
 
-// Stage the distinct (class, Th) tables the image selects, exactly as the lane kernel lays them out, and its MCU layout.
+// Stage the image's decode tables and its MCU layout.
 __device__ __forceinline__ void ph_stage(PhShared& sh, uint16_t* lutb, const DevImage& im, const DevTableSet* ts)
 {
     __syncthreads();
+    lane_stage(sh.t, lutb, im, ts);
     if (threadIdx.x == 0) ph_layout(sh, im);
-    __syncthreads();
-    const uint32_t nl = sh.nl;
-    for (uint32_t j = 0; j < nl; j++) {
-        const uint32_t slot = sh.lslot[j];
-        const uint4* s0 = reinterpret_cast<const uint4*>(ts->lut[slot]);
-        uint4* d0 = reinterpret_cast<uint4*>(lutb + j * JS_LANE_TAB);
-        for (uint32_t i = threadIdx.x; i < JS_LUT_SIZE * 2 / 16; i += blockDim.x) d0[i] = __ldg(s0 + i);
-        const uint4* s1 = reinterpret_cast<const uint4*>(ts->lut2[slot]);
-        uint4* d1 = reinterpret_cast<uint4*>(lutb + j * JS_LANE_TAB + JS_LUT_SIZE);
-        const uint32_t used = min(ts->lut2_used[slot], (uint32_t)JS_LANE_L2S);     // <= JS_LANE_L2S: the launcher refuses the batch otherwise
-        for (uint32_t i = threadIdx.x; i < used * 2 / 16; i += blockDim.x) d1[i] = __ldg(s1 + i);
-    }
-    for (uint32_t c = 0; c < im.ns; c++)
-        for (uint32_t i = threadIdx.x; i < 80; i += blockDim.x) sh.qz[c][i] = (i < 64) ? ts->qz[im.dqt[c]][i] : ((64u + (i & 7)) << 16);
     __syncthreads();
 }
 
 __device__ __forceinline__ PhTabs ph_tabs(const PhShared& sh, const uint16_t* lutb)
 {
-    PhTabs t; t.lutb = lutb; t.qz = &sh.qz[0][0]; t.blk_dc = sh.blk_dc; t.blk_ac = sh.blk_ac; t.blk_c = sh.blk_c; t.bpm = sh.bpm; t.pshift = sh.pshift;
+    PhTabs t; t.lutb = lutb; t.qz = &sh.t.qz[0][0]; t.blk_dc = sh.blk_dc; t.blk_ac = sh.blk_ac; t.blk_c = sh.blk_c; t.bpm = sh.bpm; t.pshift = sh.pshift;
     return t;
 }
 __device__ __forceinline__ PhSegs ph_segs(const DevBatch& b, const DevImage& im)

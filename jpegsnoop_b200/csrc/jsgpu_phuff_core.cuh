@@ -17,8 +17,9 @@
 //              start of every slot -> each slot is a VIRTUAL restart interval for the lane kernel (k_huff_lane<VSEG>),
 //              which then decodes every symbol exactly once, writes the coefficient rows and counts the code lengths.
 //
-// Everything in this header is plain C++ shared by the device kernels (jsgpu_phuff.cu, jsgpu_huff.cu) and by the host
-// model the CPU test-suite runs (tests/native/phuff_model.cpp): JS_HD is __host__ __device__ under nvcc.
+// Everything in this header but the shared-memory staging (device only) is plain C++ shared by the device kernels
+// (jsgpu_phuff.cu, jsgpu_huff.cu) and by the host model the CPU test-suite runs (tests/native/phuff_model.cpp): JS_HD is
+// __host__ __device__ under nvcc.
 #pragma once
 #include "jsgpu_internal.h"
 
@@ -48,6 +49,53 @@ struct PhTabs {
     const uint8_t*  blk_c;         // [bpm] its component
     uint32_t bpm, pshift;          // blocks per MCU; precision - 8 (ReadScanVal's divide, ImgDecode.cpp:1234-1238)
 };
+
+// What the lane kernel and the self-synchronising passes stage in shared memory besides the tables themselves (lane_stage).
+struct LaneTabs {
+    uint32_t qz[3][80];            // quantiser | natural index<<16 ; entries 64..79 -> dummy slots past the row
+    uint32_t li[6];                // [comp*2 + class] -> staged table index
+    uint32_t lslot[6];             // staged table index -> slot
+    uint32_t nl, pad;
+};
+
+#if defined(__CUDACC__)
+// One component's quantiser row for the decode loops: the table's entries at zig-zag positions 0..63, then no-ops (quantiser 0,
+// a dummy slot past the row) where a run carries the position beyond 63.  All threads of the CTA.
+__device__ __forceinline__ void stage_qz(uint32_t* row, const uint32_t* q)
+{
+    for (uint32_t i = threadIdx.x; i < 80; i += blockDim.x) row[i] = (i < 64) ? q[i] : ((64u + (i & 7)) << 16);
+}
+
+// Stage the decode tables of image im: its distinct (class, Th) tables, table j at lutb + j * JS_LANE_TAB, and its quantiser
+// rows.  All threads of the CTA; one barrier inside (the table list thread 0 makes), the caller synchronises before and after.
+__device__ __forceinline__ void lane_stage(LaneTabs& t, uint16_t* lutb, const DevImage& im, const DevTableSet* ts)
+{
+    if (threadIdx.x == 0) {
+        uint32_t n = 0;
+        for (uint32_t c = 0; c < im.ns; c++) for (uint32_t cls = 0; cls < 2; cls++) {
+            const uint32_t slot = cls ? im.slot_ac[c] : im.slot_dc[c];
+            uint32_t j = 0;
+            while (j < n && t.lslot[j] != slot) j++;
+            if (j == n) t.lslot[n++] = slot;
+            t.li[c * 2 + cls] = j;
+        }
+        t.nl = n;
+    }
+    __syncthreads();
+    const uint32_t nl = t.nl;
+    for (uint32_t j = 0; j < nl; j++) {
+        const uint32_t slot = t.lslot[j];
+        const uint4* s0 = reinterpret_cast<const uint4*>(ts->lut[slot]);
+        uint4* d0 = reinterpret_cast<uint4*>(lutb + j * JS_LANE_TAB);
+        for (uint32_t i = threadIdx.x; i < JS_LUT_SIZE * 2 / 16; i += blockDim.x) d0[i] = __ldg(s0 + i);
+        const uint4* s1 = reinterpret_cast<const uint4*>(ts->lut2[slot]);
+        uint4* d1 = reinterpret_cast<uint4*>(lutb + j * JS_LANE_TAB + JS_LUT_SIZE);
+        const uint32_t used = min(ts->lut2_used[slot], (uint32_t)JS_LANE_L2S);     // <= JS_LANE_L2S: the launchers refuse the batch otherwise
+        for (uint32_t i = threadIdx.x; i < used * 2 / 16; i += blockDim.x) d1[i] = __ldg(s1 + i);
+    }
+    for (uint32_t c = 0; c < im.ns; c++) stage_qz(t.qz[c], ts->qz[im.dqt[c]]);
+}
+#endif
 
 JS_HD unsigned long long ph_pack(uint32_t pos, uint32_t blk, uint32_t zz) { return (unsigned long long)pos | ((unsigned long long)blk << 32) | ((unsigned long long)zz << 40); }
 JS_HD uint32_t ph_pos(unsigned long long x) { return (uint32_t)x; }

@@ -26,10 +26,10 @@ class DecodedImage:
 class CimgDecode:
     """Mirror of the reference class (source/ImgDecode.h:284-425) driven through jsimg_*."""
 
-    def __init__(self, decode_ac=True, idct_fixedpt=True, device=0, huff_kernel=0, idct_kernel=0, device_markers=True):
+    def __init__(self, decode_ac=True, idct_fixedpt=True, device=0, huff_kernel=0, idct_kernel=0):
         self.L = B.load()
         self.h = C.c_void_p(self.L.jsimg_create())
-        self.L.jsimg_config(self.h, int(decode_ac), int(idct_fixedpt), device, huff_kernel, idct_kernel, int(device_markers))
+        self.L.jsimg_config(self.h, int(decode_ac), int(idct_fixedpt), device, huff_kernel, idct_kernel, 1)
         self._file = None
 
     def close(self):
@@ -190,7 +190,7 @@ class BatchDecoder:
     """
 
     def __init__(self, device=0, idct_fixedpt=True, decode_ac=True, huff_kernel=0, idct_kernel=0,
-                 want_histo=True, want_mcu_map=True, device_markers=True):
+                 want_histo=True, want_mcu_map=True):
         self.L = B.load()
         ctx = C.c_void_p()
         r = self.L.jsgpu_init(device, C.byref(ctx))
@@ -207,7 +207,7 @@ class BatchDecoder:
         self._ck(self.L.jsgpu_set_idct_tables(self.ctx, li.ctypes.data, lf.ctypes.data))
         self.opt = B.jsgpu_options(idct_mode=0 if idct_fixedpt else 1, decode_ac=int(decode_ac), huff_kernel=huff_kernel,
                                    idct_kernel=idct_kernel, want_histo=int(want_histo), want_mcu_map=int(want_mcu_map),
-                                   device_markers=int(device_markers), scan_err_max=0)
+                                   scan_err_max=0)
         self._ck(self.L.jsgpu_set_options(self.ctx, C.byref(self.opt)))
         self.n = 0; self.layout = None; self.descs = None; self.bitstream = None; self.nsof_pixels = 0
 

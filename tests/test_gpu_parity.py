@@ -286,18 +286,6 @@ def test_idct_table_sources_match_oracle(built, cases, tab, monkeypatch):
         assert not JC.compare(orc.decode(j), bd.fetch(i), what=("pix_y", "pix_cb", "pix_cr", "dib")), (name, tab)
 
 
-def test_host_marker_walk_equals_device_marker_scan(built, cases):
-    from jpegsnoop_b200 import BatchDecoder
-    jpegs = [j for _, j in cases]
-    outs = []
-    for dm in (True, False):
-        bd = BatchDecoder(idct_kernel=1, device_markers=dm)
-        bd.set_batch(jpegs); bd.decode(); bd.sync()
-        outs.append([bd.fetch(i) for i in range(len(jpegs))])
-    for a, b, (name, _) in zip(outs[0], outs[1], cases):
-        assert not JC.compare(a, b, what=("pix_y", "dib", "mcu_map", "dht_histo")), name
-
-
 def test_unsupported_images_in_a_batch_are_skipped(built, cases):
     """Images the reference's DecodeScanImg would refuse (here: 4-component CMYK scans) occupy no pool space, carry
     status 0x80000000 and do not disturb their neighbours — also at the start of an image range of the pipelined

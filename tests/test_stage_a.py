@@ -291,13 +291,12 @@ def _all_jpegs():
 
 @pytest.mark.gpu
 @needs_ref
-@pytest.mark.parametrize("device_markers", [True, False], ids=["device_markers", "host_walk"])
-def test_placed_files_match_the_reference_line_for_line(built, device_markers):
+def test_placed_files_match_the_reference_line_for_line(built):
     """Single-image decodes: every buffer, the whole stats row, the whole non-quiet log (scan-position and compression-ratio
-    lines included) and, for damaged files, every error line.  device_markers=False is the host walk's opinion of the bounds."""
+    lines included) and, for damaged files, every error line."""
     from jpegsnoop_b200 import CimgDecode
     o = Oracle("ref_fixed")
-    dec = CimgDecode(idct_fixedpt=True, device_markers=device_markers)
+    dec = CimgDecode(idct_fixedpt=True)
     for name, j in _all_jpegs():
         want = o.decode(j, quiet=False); wl = o.log_lines(); we = o.err_lines()
         got = dec.decode(j, quiet=False)

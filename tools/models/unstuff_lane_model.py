@@ -16,12 +16,29 @@ def byte_perm(a, b, sel):
     return r
 
 
-SELBE = []
-for t in range(16):
-    kept = [j for j in range(4) if not (t >> j) & 1]; n = len(kept); sel = 0
+def us_selector(rm, big_endian):
+    sel = 0; n = 0
     for i in range(4):
-        sel |= (kept[n - 1 - i] if i < n else 4) << (4 * i)
-    SELBE.append(sel)
+        j = 3 - i if big_endian else i
+        if not (rm >> j) & 1:
+            sel |= j << (4 * n); n += 1
+    for n in range(n, 4):
+        sel |= 4 << (4 * n)
+    return sel
+
+
+SELBE = [us_selector(t, True) for t in range(16)]
+
+
+def us_classify(prev, word, rel0, length):
+    vlo = max(0, -rel0); vhi = min(4, length - rel0)
+    vn = (((1 << vhi) - 1) & ~((1 << vlo) - 1)) & 15 if vhi > vlo else 0
+    an = (vn & ~(1 << (-rel0))) if (rel0 <= 0 and rel0 > -4) else vn
+    pw = byte_perm(prev, word, 0x6543); npw = (~pw) & M32
+    z = (~((((word & 0x7F7F7F7F) + 0x7F7F7F7F) | word | 0x7F7F7F7F))) & M32
+    f = (~((((npw & 0x7F7F7F7F) + 0x7F7F7F7F) | npw | 0x7F7F7F7F))) & M32
+    dn = (((((z & f) >> 7) * 0x00204081) & M32) >> 21) & an
+    return dn, dn | (vn ^ 15)
 
 
 def lane_unstuff(buf, s0, length):
@@ -30,15 +47,8 @@ def lane_unstuff(buf, s0, length):
     acc = 0; nacc = 0; wr = 0; nstuff = 0; prevw = 0; out = []; stuff = []
     for j in range(nwords):
         word = int.from_bytes(bytes(buf[base + 4 * j + i] if base + 4 * j + i < len(buf) else 0 for i in range(4)), "little")
-        rel0 = 4 * j - mis
-        vlo = max(0, -rel0); vhi = min(4, length - rel0)
-        vn = (((1 << vhi) - 1) & ~((1 << vlo) - 1)) & 15 if vhi > vlo else 0
-        an = (vn & ~(1 << (-rel0))) if (rel0 <= 0 and rel0 > -4) else vn
-        pw = byte_perm(prevw, word, 0x6543); npw = (~pw) & M32
-        z = (~((((word & 0x7F7F7F7F) + 0x7F7F7F7F) | word | 0x7F7F7F7F))) & M32
-        f = (~((((npw & 0x7F7F7F7F) + 0x7F7F7F7F) | npw | 0x7F7F7F7F))) & M32
-        dn = (((((z & f) >> 7) * 0x00204081) & M32) >> 21) & an
-        rm = dn | (vn ^ 15); cnt = 4 - popc(rm)
+        dn, rm = us_classify(prevw, word, 4 * j - mis, length)
+        cnt = 4 - popc(rm)
         d = dn
         while d:
             jj = (d & -d).bit_length() - 1; d &= d - 1
