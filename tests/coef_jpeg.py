@@ -6,9 +6,11 @@ quantiser 1..65535 (16-bit DQT entries where needed), DC and AC sizes up to 15 a
 sizes, so that a code plus its value bits is a 30-31-bit step.  Neither Pillow nor tests/mini_jpeg.py can write these.
 
 `expected` is the decode of such a file by the reference's arithmetic (ImgDecode.cpp ReadScanVal, DecodeIdctSet,
-DecodeIdctCalcFixedpt / DecodeIdctCalcFloat, SetFullRes, ConvertYCCtoRGBFastFloat, the block-DC maps) for the layouts the
-fused kernels decode: 4:4:4, 4:2:2, 4:2:0 and greyscale.  It uses the IDCT tables the oracle hands out, nothing else
-from the reference."""
+DecodeIdctCalcFixedpt / DecodeIdctCalcFloat, SetFullRes, ConvertYCCtoRGBFastFloat, the block-DC maps) for every layout
+whose components each have a sampling factor of 1 or the maximum in each direction (4:4:4, 4:2:2, 4:2:0, 4:1:1, 4:4:0,
+2x4 + 2x1, 4x3 + 1x3 ... and greyscale): there no two blocks of a component overlap.  It uses the IDCT tables the oracle
+hands out, nothing else from the reference.  `expected_stats` restates the brightest-pixel and average-luma statistics
+CalcChannelPreviewFull derives from those maps."""
 import numpy as np
 
 from mini_jpeg import ZZ, BitWriter, bits_from_lengths, canonical_codes, _seg
@@ -252,7 +254,7 @@ def expected(spec, idct_fixed, li, lf, decode_ac=True):
     img_x, img_y = mxn * mcu_w, myn * mcu_h
     blk_xmax, blk_ymax = mxn * hmax, myn * vmax
     for h, v in samp:
-        assert (h, v) in ((hmax, vmax), (1, 1)), "expected() covers the fused layouts only"
+        assert h in (1, hmax) and v in (1, vmax), "expected() covers layouts whose factors are 1 or the maximum only"
     div = 1 << (P - 8)
     e = Expected()
     e.geom = np.array([mcu_w, mcu_h, mxn, myn, blk_xmax, blk_ymax, img_x, img_y], np.uint32)
@@ -324,3 +326,30 @@ def expected(spec, idct_fixed, li, lf, decode_ac=True):
         e.blk_dc = (dcmaps[0], None, None)
         e.dib = ycc_to_bgra(maps[0], z, z)[::-1].copy()
     return e
+
+
+def expected_stats(e):
+    """The reference's stats[0:10] (avgY, avgY valid, brightest Y, Cb, Cr, R, G, B, its MCU x, y) for an `expected` result:
+    CalcChannelPreviewFull (ImgDecode.cpp:4693-4730, 4813-4819) walks the padded maps in raster order and keeps the first
+    strict maximum of raw Y, starting from -32768, so an image whose Y is -32768 everywhere keeps the initial values at pixel 0;
+    the luma sum is a 32-bit unsigned and the divisor is (Wp + 1)(Hp + 1)."""
+    mcu_w, mcu_h, Wp, Hp = int(e.geom[0]), int(e.geom[1]), int(e.geom[6]), int(e.geom[7])
+    y = np.asarray(e.pix_y, np.int64).ravel()
+    idx = int(np.argmax(y))
+    if y[idx] == -32768:
+        by = bcb = bcr = -32768; idx = 0
+    else:
+        by = int(y[idx])
+        bcb = int(np.asarray(e.pix_cb).ravel()[idx]) if e.pix_cb is not None else 0
+        bcr = int(np.asarray(e.pix_cr).ravel()[idx]) if e.pix_cr is not None else 0
+    b, g, r, _ = (int(v) for v in ycc_to_bgra(by, bcb, bcr))
+    s = int((np.clip(y >> 3, -128, 127) + 128).sum()) & 0xFFFFFFFF
+    avg = s // ((Wp + 1) * (Hp + 1))
+    return np.array([avg, 1, by, bcb, bcr, r, g, b, (idx % Wp) // mcu_w, (idx // Wp) // mcu_h], np.int32)
+
+
+def device_stats(st):
+    """The reference's stats[0:10] layout from the device's 16-word stats row (include/jsgpu.h: [2] m_nAvgY, [3:11] the
+    brightest pixel's Y, Cb, Cr, R, G, B and its MCU x, y); the valid flag is set by every decode."""
+    st = np.asarray(st, np.int64)
+    return np.concatenate([[st[2], 1], st[3:11]]).astype(np.int32)
