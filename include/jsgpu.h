@@ -368,6 +368,22 @@ int jsgpu_decode_batch_host(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32
                             const uint8_t* host_bitstream, uint64_t bitstream_bytes,
                             const jsgpu_host_outputs* out);
 
+/* --- byte-pattern search (Tools -> Search Executable for DQT, JPEGsnoopDoc.cpp:1233-1529) ---------------------------------
+ * Replaces the Doc's loop "start = 0; while CwindowBuf::BufSearchX(start, pat, L, forward) finds p: report p; start = p + 1"
+ * (WindowBuf.cpp:243-331) for `npat` patterns at once, in one streaming pass over the n bytes at `data` (host memory).
+ * Pattern k is lens[k] bytes (8..256) at patterns + lens[0] + .. + lens[k-1].  It reports exactly what that loop reports:
+ * every p where the pattern matches byte for byte, 1 <= p <= n - 2 lens[k] + 2 (the reference never reports offset 0 and
+ * stops short of the last 2 L - 2 bytes), and p - 1 was not reported itself (a run of overlapping matches reports every
+ * other one).  counts[k] receives pattern k's full count; pos receives at most `cap` positions, ascending per pattern,
+ * pattern k's after pattern k-1's.  Files of 2^32 bytes or more are refused (JSGPU_EINVAL): the reference's offsets are 32-bit.
+ * The file is streamed in chunks (64 MiB; the environment variable JSGPU_SEARCH_CHUNK_BYTES, read at every call, changes
+ * that) through pinned double buffers on the search's own streams; the batch of the context is left untouched.  Synchronous. */
+#define JSGPU_SEARCH_MAX_PATTERNS 32
+#define JSGPU_SEARCH_MIN_LEN      8
+#define JSGPU_SEARCH_MAX_LEN      256
+int jsgpu_search_bytes(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, const uint8_t* patterns, const uint32_t* lens, uint32_t npat,
+                       uint64_t* counts, uint32_t* pos, uint64_t cap);
+
 /* Pinned host memory helpers (for callers that want true async copies). */
 void* jsgpu_host_alloc(uint64_t bytes);
 void  jsgpu_host_free(void* p);

@@ -74,6 +74,13 @@ int    jsimg_ExportTiff(jsimg*, const char* path, unsigned mode);
 /* FileTiff::WriteFile on a caller-made sample array (no device involved); 1 on success */
 int    jsimg_tiff_write(const char* path, int ycc, int b16, const void* data, unsigned w, unsigned h);
 
+/* Tools -> Search Executable for DQT (CJPEGsnoopDoc::OnToolsSearchexecutablefordqt, JPEGsnoopDoc.cpp:1233-1529) over the n bytes
+ * at `data` (exe_path names them in the report).  With `analysed` set, the handle's decoder stands for the analysed JPEG
+ * (analysed_path): table 0 as GetDqtEntry(0, .) holds it is searched next to the JPEG standard's.  The report goes to the log,
+ * line for line and kind for kind as the reference writes it; every search runs on the GPU (jsgpu_search_bytes) in one pass.
+ * Returns 0, or a negative JSGPU_E* code after one error line and no report (no CUDA device; files of 2^32 bytes or more). */
+int    jsimg_search_dqt(jsimg*, const uint8_t* data, uint64_t n, const char* exe_path, int analysed, const char* analysed_path);
+
 /* log access (error convention: failures are log lines, ImgDecode.cpp:2755-2758 etc.) */
 int    jsimg_log_count(jsimg*, int kind /*0 line,1 hdr,2 warn,3 err,4 good,-1 all*/);
 const char* jsimg_log_line(jsimg*, int kind, int index);

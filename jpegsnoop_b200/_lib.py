@@ -102,7 +102,7 @@ JSGPU_SYMBOLS = [
     "jsgpu_batch_begin", "jsgpu_batch_layout", "jsgpu_batch_pools", "jsgpu_batch_upload", "jsgpu_batch_decode",
     "jsgpu_batch_download", "jsgpu_batch_stage_ms", "jsgpu_timer_start", "jsgpu_timer_stop", "jsgpu_batch_launches", "jsgpu_batch_selfsync_info", "jsgpu_batch_checksums", "jsgpu_batch_errors", "jsgpu_decode_batch_host",
     "jsgpu_host_alloc", "jsgpu_host_free", "jsgpu_host_copy_rate", "jsgpu_set_preview", "jsgpu_batch_preview", "jsgpu_batch_colour_stats", "jsgpu_batch_export", "jsgpu_set_detail", "jsgpu_batch_detail",
-    "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices"]
+    "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices", "jsgpu_search_bytes"]
 JSIMG_SYMBOLS = [
     "jsimg_create", "jsimg_destroy", "jsimg_config", "jsimg_set_file", "jsimg_overlay_install", "jsimg_overlay_remove_all", "jsimg_Reset", "jsimg_ResetState",
     "jsimg_SetDqtEntry", "jsimg_SetDqtTables", "jsimg_GetDqtEntry", "jsimg_SetDhtTables", "jsimg_SetDhtEntry",
@@ -112,7 +112,8 @@ JSIMG_SYMBOLS = [
     "jsimg_GetDhtHisto", "jsimg_GetGeometry", "jsimg_GetStats", "jsimg_GetIdctTables", "jsimg_GetStageMs", "jsimg_GetScanStatus",
     "jsimg_log_count", "jsimg_log_line", "jsimg_log_clear", "jsimg_walk_jpeg", "jsimg_decode_jpeg", "jsimg_parse_jpeg",
     "jsimg_config_histo", "jsimg_SetPreviewMode", "jsimg_GetPreviewMode", "jsimg_SetPreviewYccOffset", "jsimg_GetPreviewYccOffset",
-    "jsimg_GetStatClip", "jsimg_GetHistoRanges", "jsimg_GetCcHisto", "jsimg_GetHistoYFull", "jsimg_GetHistoDib", "jsimg_ExportTiff", "jsimg_tiff_write", "jsimg_SetDetailVlc", "jsimg_GetDetailVlc"]
+    "jsimg_GetStatClip", "jsimg_GetHistoRanges", "jsimg_GetCcHisto", "jsimg_GetHistoYFull", "jsimg_GetHistoDib", "jsimg_ExportTiff", "jsimg_tiff_write", "jsimg_SetDetailVlc", "jsimg_GetDetailVlc",
+    "jsimg_search_dqt"]
 
 _lib = None
 
@@ -166,6 +167,8 @@ def load():
     L.jsgpu_batch_detail_info.argtypes = [vp, vp]
     L.jsgpu_batch_detail_events.argtypes = [vp, u32, u32, vp]
     L.jsgpu_batch_detail_matrices.argtypes = [vp, u32, u32, vp]
+    L.jsgpu_search_bytes.argtypes = [vp, vp, u64, vp, vp, u32, vp, vp, u64]
+    L.jsimg_search_dqt.argtypes = [vp, vp, u64, C.c_char_p, i32, C.c_char_p]
     L.jsimg_SetDetailVlc.argtypes = [vp, i32, u32, u32, u32]; L.jsimg_SetDetailVlc.restype = None
     L.jsimg_GetDetailVlc.argtypes = [vp] + [C.POINTER(u32)] * 4; L.jsimg_GetDetailVlc.restype = None
     L.jsimg_config_histo.argtypes = [vp, i32, i32, i32]; L.jsimg_config_histo.restype = None

@@ -6,14 +6,14 @@
 #include "ImgDecode.h"
 #include "JfifWalk.h"
 
-static const unsigned kZigZag[64] = {      // zig-zag position -> natural index (T.81 Figure A.6)
+const unsigned kJfifZigZag[64] = {
      0, 1, 8,16, 9, 2, 3,10, 17,24,32,25,18,11, 4, 5, 12,19,26,33,40,48,41,34, 27,20,13, 6, 7,14,21,28,
     35,42,49,56,57,50,43,36, 29,22,15,23,30,37,44,51, 58,59,52,45,38,31,39,46, 53,60,61,54,47,55,62,63 };
 
 int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n)
 {
     unsigned unzz[64];
-    for (unsigned i = 0; i < 64; i++) unzz[kZigZag[i]] = i;
+    for (unsigned i = 0; i < 64; i++) unzz[kJfifZigZag[i]] = i;
     pImgDec->ResetState();
     if (n < 4 || d[0] != 0xFF || d[1] != 0xD8) return JFIFWALK_ENOTJPEG;
     uint64_t p = 2;
@@ -36,7 +36,7 @@ int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n)
                 for (unsigned k = 0; k < 64; k++) {                 // file order is zig-zag (JfifDecode.cpp:4576-4584)
                     if (q >= e) return JFIFWALK_ETRUNC;
                     unsigned v = d[q++]; if (Pq) { if (q >= e) return JFIFWALK_ETRUNC; v = (v << 8) | d[q++]; }
-                    tbl[kZigZag[k]] = v;
+                    tbl[kJfifZigZag[k]] = v;
                 }
                 for (unsigned i = 0; i < 64; i++) pImgDec->SetDqtEntry(Tq, i, unzz[i], (unsigned short)tbl[i]);   // :4648
             }

@@ -9,3 +9,5 @@ class CimgDecode;
 // Walk the markers of the first frame of a JPEG and issue CjfifDecode's setter sequence on pImgDec.
 // Returns the file offset of the first entropy-coded byte of the first scan (>0) or a JFIFWALK_E* code.
 int JfifWalk(CimgDecode* pImgDec, const uint8_t* data, uint64_t n);
+// zig-zag position -> natural index (T.81 Figure A.6; the permutation of the reference's glb_anZigZag)
+extern const unsigned kJfifZigZag[64];

@@ -3,12 +3,14 @@
 #include "ImgDecode.h"
 #include "TiffExport.h"
 #include "JfifWalk.h"
+#include "DqtSearch.h"
 #include <cstring>
 
 struct jsimg {
     CDocLog log; CwindowBuf wbuf; CSnoopConfig cfg; CimgDecode* dec;
+    jsgpu_ctx* search = nullptr;        // the byte-pattern search's device context (jsimg_search_dqt), created on first use
     jsimg() : dec(new CimgDecode(&log, &wbuf, &cfg)) {}
-    ~jsimg() { delete dec; }
+    ~jsimg() { delete dec; if (search) jsgpu_free(search); }
 };
 
 extern "C" {
@@ -87,6 +89,10 @@ int jsimg_decode_jpeg(jsimg* h, const uint8_t* d, uint64_t n, int quiet)
     if (start < 0) return start;
     h->dec->DecodeScanImg((unsigned)start, true, quiet != 0);       // JfifDecode.cpp:5299
     return start;
+}
+int jsimg_search_dqt(jsimg* h, const uint8_t* d, uint64_t n, const char* exe_path, int analysed, const char* analysed_path)
+{
+    return DqtSearch(&h->log, &h->search, h->cfg.nCudaDevice, analysed ? h->dec : nullptr, d, n, exe_path, analysed_path);
 }
 int jsimg_parse_jpeg(const uint8_t* d, uint64_t n, jsgpu_tables* t, jsgpu_image_desc* desc)
 {

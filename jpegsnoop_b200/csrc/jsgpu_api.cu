@@ -76,6 +76,7 @@ struct jsgpu_ctx {
     DevBuf d_dt_scratch;                     // [16] counters (JsDetailOut::hdr), [136] the walk's code-length histogram, then the
                                              // parallel path's per-MCU event counts / offsets and last top-up points
     bool dt_parallel = false; JsDetailRange dt_range = {0, 0, 0, 0, 0}; JsDetailOut dt_out = {};
+    JsSearch* search = nullptr;              // jsgpu_search_bytes: own streams, staging and device buffers (not the batch pools)
 };
 
 static int fail(jsgpu_ctx* c, int code, const char* fmt, ...)
@@ -152,6 +153,7 @@ void jsgpu_free(jsgpu_ctx* ctx)
     if (!ctx) return;
     for (jsgpu_ctx* k : ctx->kids) jsgpu_free(k);
     ctx->kids.clear();
+    js_search_free(ctx->search);
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     DevBuf* bufs[] = { &ctx->d_ctab, &ctx->d_li, &ctx->d_lf, &ctx->d_sym, &ctx->d_tables, &ctx->d_img, &ctx->d_items, &ctx->d_litems, &ctx->d_tiles, &ctx->d_ubits, &ctx->d_seg64, &ctx->d_ph, &ctx->d_rowtab, &ctx->d_ex, &ctx->d_cstats, &ctx->d_rowclip, &ctx->d_dt_ev, &ctx->d_dt_mat, &ctx->d_dt_scratch, &ctx->d_mc, &ctx->d_bits, &ctx->d_seg,
@@ -1064,6 +1066,21 @@ int jsgpu_host_copy_rate(jsgpu_ctx* ctx, int direction, uint64_t bytes, int reps
     if (e != cudaSuccess) return fail(ctx, JSGPU_ECUDA, "copy-rate probe failed: %s", cudaGetErrorString(e));
     *gbs = best;
     return JSGPU_OK;
+}
+
+int jsgpu_search_bytes(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, const uint8_t* patterns, const uint32_t* lens, uint32_t npat,
+                       uint64_t* counts, uint32_t* pos, uint64_t cap)
+{
+    if (!ctx) return JSGPU_EINVAL;
+    if (!counts || !lens || !patterns || (n && !data) || (cap && !pos) || npat == 0 || npat > JSGPU_SEARCH_MAX_PATTERNS)
+        return fail(ctx, JSGPU_EINVAL, "jsgpu_search_bytes: bad arguments (npat %u, 1..%d patterns)", npat, JSGPU_SEARCH_MAX_PATTERNS);
+    for (uint32_t k = 0; k < npat; k++)
+        if (lens[k] < JSGPU_SEARCH_MIN_LEN || lens[k] > JSGPU_SEARCH_MAX_LEN)
+            return fail(ctx, JSGPU_EINVAL, "jsgpu_search_bytes: pattern %u is %u bytes (%d..%d)", k, lens[k], JSGPU_SEARCH_MIN_LEN, JSGPU_SEARCH_MAX_LEN);
+    if (n >> 32)
+        return fail(ctx, JSGPU_EINVAL, "jsgpu_search_bytes: %llu bytes: files of 2^32 bytes or more do not fit 32-bit offsets",
+                    (unsigned long long)n);
+    return js_search_run(&ctx->search, ctx->device, ctx->sm_count, data, n, patterns, lens, npat, counts, pos, cap, ctx->err);
 }
 
 void* jsgpu_host_alloc(uint64_t bytes) { void* p = nullptr; if (cudaMallocHost(&p, bytes) != cudaSuccess) return nullptr; return p; }

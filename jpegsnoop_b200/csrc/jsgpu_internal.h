@@ -3,6 +3,7 @@
 #pragma once
 #include <stdint.h>
 #include <cuda_runtime.h>
+#include <string>
 #include "../../include/jsgpu.h"
 
 #define JS_LUT_BITS   10                 // direct Huffman look-up width (reference uses 9: ImgDecode.h:96)
@@ -195,6 +196,11 @@ int js_launch_finalize_stats(const DevBatch& b, cudaStream_t s);    // brightest
 // CalcChannelPreviewFull with non-default settings: clipping/histogram conversion, channel selection, YCC shift (jsgpu_preview.cu)
 int js_launch_preview(const DevBatch& b, const jsgpu_preview& pv, jsgpu_colour_stats* st, uint32_t* rowclip, uint64_t rows_total,
                       uint32_t max_hp, int sm_count, cudaStream_t s);
+// byte-pattern search (jsgpu_search.cu): its own streams and buffers, created on first use and kept by the context
+struct JsSearch;
+int  js_search_run(JsSearch** s, int device, int sm_count, const uint8_t* data, uint64_t n, const uint8_t* pats, const uint32_t* lens,
+                   uint32_t npat, uint64_t* counts, uint32_t* pos, uint64_t cap, std::string& err);
+void js_search_free(JsSearch* s);
 #define JSGPU_CK_WORDS_INTERNAL 12   // == JSGPU_CK_WORDS (include/jsgpu.h)
 int js_launch_checksums(const DevBatch& b, unsigned long long* ck, cudaStream_t s);
 int js_launch_finalize_emptied(const DevBatch& b, cudaStream_t s);   // after js_launch_finalize: drained-interval MCU map entries

@@ -113,6 +113,33 @@ class CimgDecode:
         """Export-to-TIFF of the decoded image (mode 0 RGB 8-bit, 1 RGB 16-bit, 2 YCC 8-bit), JPEGsnoopDoc.cpp:2008-2193."""
         return bool(self.L.jsimg_ExportTiff(self.h, str(path).encode(), mode))
 
+    def search_dqt(self, data, exe_path, analysed=False, analysed_path=""):
+        """Tools -> Search Executable for DQT over `data` (JPEGsnoopDoc.cpp:1233-1529), on the GPU.  With `analysed`, this
+        decoder's table 0 (from the last walk/decode) is searched next to the JPEG standard's.  The report goes to the log
+        (log_lines()); returns {(ordering, set, layout): [positions]} for every search the report lists: ordering 0
+        pre-zigzag / 1 post-zigzag, set 0 the standard table / 1 the analysed one, layout 0..4 = 1-byte, 2-byte,
+        2-byte swapped, 4-byte, 4-byte swapped (a skipped 1-byte search is absent).  Raises JsgpuError on failure."""
+        buf = np.frombuffer(data, np.uint8) if isinstance(data, np.ndarray) else np.frombuffer(bytes(data), np.uint8)
+        n0 = self.L.jsimg_log_count(self.h, -1)
+        r = self.L.jsimg_search_dqt(self.h, buf.ctypes.data, buf.size, str(exe_path).encode(), int(analysed), str(analysed_path).encode())
+        lines = self.log_lines()[n0:]
+        if r != 0:
+            raise JsgpuError(f"jsimg_search_dqt failed ({r}): {lines}")
+        found, key, zz, ts = {}, None, -1, -1
+        for s in lines:
+            if s.startswith("    DQT Ordering: "):
+                zz += 1; ts = -1
+            elif s.startswith("      Matching ["):
+                ts += 1
+            elif s.startswith("        Searching patterns with "):
+                w = int(s.split("with ")[1].split("-byte")[0]); swap = s.endswith("byteswap")
+                key = (zz, ts, {1: 0, 2: 1, 4: 3}[w] + int(swap)); found[key] = []
+            elif s.startswith("          DQT Table is not baseline"):
+                del found[key]
+            elif s.startswith("          Found @ 0x"):
+                found[key].append(int(s.split("0x")[1], 16))
+        return found
+
     def bitmap(self):
         g = np.zeros(8, np.uint32); self.L.jsimg_GetGeometry(self.h, g.ctypes.data)
         p = self.L.jsimg_GetBitmapPtr(self.h)
@@ -280,6 +307,25 @@ class BatchDecoder:
     def host_copy_rate(self, direction=1, nbytes=1 << 30, reps=3):
         """GB/s of a plain cudaMemcpyAsync between pinned host memory and this GPU (1 = device->host)."""
         g = C.c_float(0); self._ck(self.L.jsgpu_host_copy_rate(self.ctx, direction, nbytes, reps, C.byref(g))); return float(g.value)
+
+    def search_bytes(self, data, patterns, cap=None):
+        """jsgpu_search_bytes: every position the reference's repeated BufSearchX loop reports for each pattern (8..256 bytes,
+        at most 32) in `data` (bytes or a uint8 array).  Returns (counts uint64 [npat], [positions uint32 array per pattern]);
+        with `cap`, at most cap positions are returned in all (counts stay complete)."""
+        buf = data if isinstance(data, np.ndarray) else np.frombuffer(bytes(data), np.uint8)
+        pats = [np.frombuffer(bytes(p), np.uint8) for p in patterns]
+        cat = np.concatenate(pats) if pats else np.zeros(0, np.uint8)
+        lens = np.array([p.size for p in pats], np.uint32)
+        counts = np.zeros(len(pats), np.uint64)
+        if cap is None:                       # count first, then fetch everything
+            self._ck(self.L.jsgpu_search_bytes(self.ctx, buf.ctypes.data, buf.size, cat.ctypes.data, lens.ctypes.data, len(pats),
+                                               counts.ctypes.data, None, 0))
+            cap = int(counts.sum())
+        pos = np.zeros(max(int(cap), 1), np.uint32)
+        self._ck(self.L.jsgpu_search_bytes(self.ctx, buf.ctypes.data, buf.size, cat.ctypes.data, lens.ctypes.data, len(pats),
+                                           counts.ctypes.data, pos.ctypes.data, int(cap)))
+        first = np.concatenate([[0], np.cumsum(counts.astype(np.int64))])
+        return counts, [pos[min(first[k], cap):min(first[k + 1], cap)].copy() for k in range(len(pats))]
 
     def scan_errors(self, i):
         """jsgpu_scan_errors of image i (only for images whose status carries JSGPU_ST_EXACT = 0x40000000)."""
