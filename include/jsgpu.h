@@ -136,6 +136,7 @@ typedef struct {
 #define JSGPU_STAT_END_ALIGN 13
 #define JSGPU_STAT_END_MARK  14  /* file position of the marker that ends the scan (BuffAddByte logs it, ImgDecode.cpp:1527-1543) */  /* "Next position in scan buffer" and compression-ratio lines (ImgDecode.cpp:3659-3726)  */
 #define JSGPU_STAT_WORDS     16
+#define JSGPU_HISTO_WORDS    136 /* dht_histo words per image: [2][4][17]                      */
 
 /* Output selectors for jsgpu_batch_download */
 #define JSGPU_OUT_PIX_Y   0
@@ -200,7 +201,8 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx);
 int jsgpu_batch_download(jsgpu_ctx* ctx, int which, uint32_t image, void* host_dst, uint64_t bytes);
 /* Device-side times (ms) of the last jsgpu_batch_decode, measured with CUDA events on the
  * context stream: [0] marker scan, [1] Huffman, [2] IDCT+colour, [3] stats/map finalise,
- * [4] total.  Forces a sync. */
+ * [4] total.  Forces a sync.  JSGPU_ESTATE unless the context's current batch was decoded on
+ * it (not after a jsgpu_decode_batch_host that was cut into image ranges). */
 int jsgpu_batch_stage_ms(jsgpu_ctx* ctx, float* ms5);
 /* Device stopwatch on the context stream (CUDA events): start records an event, stop records a
  * second one, synchronises on it and returns the elapsed milliseconds. */
@@ -354,11 +356,14 @@ int jsgpu_batch_export(jsgpu_ctx* ctx, uint32_t image, int mode, void* host_out,
 /* One-call end-to-end form: host bitstream in, host outputs out (any pointer may be NULL to
  * skip that output).  Output buffers hold the images back to back in batch order using the
  * element offsets of jsgpu_batch_layout.  Small batches run H2D, decode and D2H on the context
- * stream.  Large ones (>= 16 images and >= 64 MB of bitstream, images laid out in increasing,
- * 16-byte aligned scan offsets) are cut into 8 image ranges, each with its own stream and device
- * pools, so the device-to-host copy of one range overlaps upload and decode of the next; afterwards
- * this context holds the batch layout and statuses only (jsgpu_batch_layout works,
- * jsgpu_batch_download / jsgpu_batch_pools return JSGPU_ESTATE: the data already is in `out`). */
+ * stream, and the context keeps the decoded batch as jsgpu_batch_decode leaves it.  Large ones
+ * (>= 16 images and >= 64 MB of bitstream, images laid out in increasing, 16-byte aligned scan
+ * offsets) are cut into 8 image ranges, each with its own stream and device pools, so the
+ * device-to-host copy of one range overlaps upload and decode of the next.  From the moment such a
+ * batch is planned, this context holds its layout only, and after the decode the statuses:
+ * jsgpu_batch_layout works; every other batch query (download, pools, stage_ms, checksums, errors,
+ * export, preview ...) returns JSGPU_ESTATE, also when a range failed, until the next
+ * jsgpu_batch_begin.  The data already is in `out`. */
 typedef struct {
     int16_t* pix_y; int16_t* pix_cb; int16_t* pix_cr; uint8_t* dib;
     int16_t* blk_y; int16_t* blk_cb; int16_t* blk_cr; uint32_t* mcu_map;

@@ -60,7 +60,7 @@ void jsimg_LookupFilePosPix(jsimg* h, unsigned px, unsigned py, unsigned* by, un
 void jsimg_LookupBlkYCC(jsimg* h, unsigned bx, unsigned by, int* y, int* cb, int* cr) { h->dec->LookupBlkYCC(bx, by, *y, *cb, *cr); }
 const uint32_t* jsimg_GetMcuFileMap(jsimg* h) { return h->dec->GetMcuFileMap(); }
 const int16_t* jsimg_GetBlkDcMap(jsimg* h, unsigned ch) { return h->dec->GetBlkDcMap(ch); }
-void jsimg_GetDhtHisto(jsimg* h, uint32_t* out) { memcpy(out, h->dec->GetDhtHisto(), 2 * 4 * 17 * sizeof(uint32_t)); }
+void jsimg_GetDhtHisto(jsimg* h, uint32_t* out) { memcpy(out, h->dec->GetDhtHisto(), JSGPU_HISTO_WORDS * sizeof(uint32_t)); }
 void jsimg_GetGeometry(jsimg* h, unsigned* out8) { h->dec->GetGeometry(out8); }
 void jsimg_GetStats(jsimg* h, int32_t* o)
 {

@@ -20,6 +20,10 @@
 
 struct DevBuf {
     void* p = nullptr; size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
     cudaError_t reserve(size_t n) {
         if (n <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -29,7 +33,46 @@ struct DevBuf {
         if (e == cudaSuccess) cap = want;
         return e;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+};
+
+// Lays out consecutive arrays in one pool.  Run once with base == nullptr to measure the bytes to reserve, then on the
+// reserved block to bind the pointers; align(a) counts a whole `a` bytes while measuring (the most it can skip).
+struct Carve {
+    uint8_t* base; size_t off = 0;
+    template <class T> void take(T*& p, uint64_t n) { p = base ? (T*)(base + off) : nullptr; off += n * sizeof(T); }
+    void align(size_t a) { off = base ? (off + a - 1) / a * a : off + a; }
+    void skip(size_t bytes) { off += bytes; }
+};
+template <class Layout> static cudaError_t carve(DevBuf& pool, Layout lay)
+{
+    Carve m{nullptr}; lay(m);
+    const cudaError_t e = pool.reserve(m.off);
+    if (e == cudaSuccess) { Carve c{(uint8_t*)pool.p}; lay(c); }
+    return e;
+}
+
+// Everything jsgpu_batch_begin derives from the image descriptors, on the host (plan_batch).
+struct BatchPlan {
+    std::vector<DevImage> img;
+    std::vector<jsgpu_image_layout> layout;
+    std::vector<uint2> items;                // Huffman warp kernel: [all | without self-synchronised images]
+    std::vector<uint2> litems;               // lane kernel: [all | without ... | slots of the self-synchronised images]
+    uint32_t n_items = 0, n_items_np = 0, n_litems = 0, n_litems_np = 0, n_vitems = 0;
+    std::vector<uint4> tiles;                // fused IDCT tiles grouped by chroma replication class
+    uint32_t tcls_first[3] = {}, tcls_count[3] = {}, plane_bytes = 0;
+    std::vector<uint32_t> mc_img;            // image of every 4096-byte chunk (marker scan)
+    // pool totals in elements (pix, blk: int16; dib: bytes; mcu, histo, stats: words), and the other sizes of the batch
+    uint64_t bits_len = 0, pix = 0, dib = 0, blk = 0, mcu = 0, histo = 0, stats = 0;
+    uint64_t coef_rows = 0, max_scan_len = 0, ubits = 0, ph = 0, rt = 0, cs = 0, rows = 0;
+    uint32_t nseg = 0, nseg_np = 0, n_psync = 0, max_cs = 0, max_hp = 0, n_std = 0, n_nonstd = 0;
+};
+
+// What the context holds of its batch.  The order matters: from JS_PLANNED on the device pools are bound.
+enum BatchState {
+    JS_NO_BATCH,
+    JS_LAYOUT_ONLY,     // the chunked jsgpu_decode_batch_host: layout and statuses here, the device pools are the chunk contexts'
+    JS_PLANNED,         // jsgpu_batch_begin: pools reserved and bound
+    JS_DECODED,         // jsgpu_batch_decode: the outputs are resident on the device
 };
 
 struct jsgpu_ctx {
@@ -50,43 +93,69 @@ struct jsgpu_ctx {
     uint32_t nsets = 0;
     std::vector<std::array<uint32_t, JS_NSLOT>> set_l2;   // per table set and slot: second-level entries used (0xffffffff = overflowed)
     // batch state
-    bool planned = false, decoded = false;
-    std::vector<DevImage> himg;
-    std::vector<jsgpu_image_layout> layout;
+    BatchState state = JS_NO_BATCH;
+    BatchPlan plan;
     DevBatch batch;
-    uint64_t bits_len = 0, pix_total = 0, dib_total = 0, blk_total = 0, mcu_total = 0, coef_rows = 0;
-    uint64_t max_scan_len = 0, ubits_total = 0, ph_total = 0, rt_total = 0;
-    uint32_t nseg_np = 0, n_psync = 0, max_cs = 0; uint64_t cs_total = 0;
-    uint32_t n_nonstd = 0, n_std = 0;
     int launches = 0;
     // host copies of the configuration, replayed into the chunk contexts of jsgpu_decode_batch_host
     std::vector<jsgpu_tables> h_sets; std::vector<int32_t> h_li; std::vector<float> h_lf;
     std::vector<jsgpu_ctx*> kids;            // chunk contexts (own stream and pools), created on first use
-    bool plan_only = false;                  // batch_begin computes the layout only (the chunk contexts own the device pools)
-    bool layout_only = false;                // ... and that is all this context currently holds: upload/decode need a new batch_begin
-    bool host_delivered = false;             // the last decode went straight to host buffers: nothing to download from this context
-    float ms[5] = {0, 0, 0, 0, 0};
     // CalcChannelPreviewFull settings (jsgpu_set_preview) and the statistics of the last preview pass
     jsgpu_preview pv = {0, 0, 1, 0, 0, 0, 0, 0, JSGPU_MAX_YCC_WARN, 0, 0, 0, 0};
-    DevBuf d_mc; uint32_t mc_total = 0;      // marker-scan chunk arrays
-    DevBuf d_cstats, d_rowclip; uint64_t rows_total = 0; uint32_t max_hp = 0; bool pv_done = false;
+    DevBuf d_mc;                             // marker-scan chunk arrays
+    DevBuf d_cstats, d_rowclip; bool pv_done = false;
     // "Detailed Decode" request (jsgpu_set_detail) and the dump of the last decode
     jsgpu_detail dtl = {0, 0, 0, 0, 0}; bool dt_done = false;
     DevBuf d_dt_ev, d_dt_mat;                // events and matrices, sized at each decode
-    DevBuf d_dt_scratch;                     // [16] counters (JsDetailOut::hdr), [136] the walk's code-length histogram, then the
+    DevBuf d_dt_scratch;                     // [16] counters (JsDetailOut::hdr), [JSGPU_HISTO_WORDS] the walk's code-length histogram, then the
                                              // parallel path's per-MCU event counts / offsets and last top-up points
     bool dt_parallel = false; JsDetailRange dt_range = {0, 0, 0, 0, 0}; JsDetailOut dt_out = {};
     JsSearch* search = nullptr;              // jsgpu_search_bytes: own streams, staging and device buffers (not the batch pools)
 };
 
-static int fail(jsgpu_ctx* c, int code, const char* fmt, ...)
+static int vfail(std::string& err, int code, const char* fmt, va_list ap)
 {
     char buf[512];
-    va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-    if (c) c->err = buf;
+    vsnprintf(buf, sizeof buf, fmt, ap);
+    err = buf;
     return code;
 }
+static int fail(std::string& err, int code, const char* fmt, ...) { va_list ap; va_start(ap, fmt); vfail(err, code, fmt, ap); va_end(ap); return code; }
+static int fail(jsgpu_ctx* c, int code, const char* fmt, ...) { va_list ap; va_start(ap, fmt); vfail(c->err, code, fmt, ap); va_end(ap); return code; }
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(ctx, (e_ == cudaErrorMemoryAllocation) ? JSGPU_ENOMEM : JSGPU_ECUDA, "%s failed: %s", #call, cudaGetErrorString(e_)); } while (0)
+static const char* const HOST_DELIVERED = "the last batch was delivered to host buffers by jsgpu_decode_batch_host";
+
+// The ten per-image outputs, indexed by JSGPU_OUT_*.  A pool holds the images back to back in batch order: image i's
+// elements start at its DevImage offset `off`, or at i * count for the fixed-size outputs (off == nullptr).
+struct JsOutput {
+    size_t dev, host;                            // offsetof its pool pointer in DevBatch and in jsgpu_host_outputs (= jsgpu_pools)
+    uint32_t elem;                               // bytes per element
+    bool chroma;                                 // absent from a one-component scan
+    uint64_t DevImage::* off;
+    uint64_t (*count)(const DevImage& im);       // elements of one image
+    uint64_t BatchPlan::* total;                 // elements of the pool
+};
+static uint64_t js_npx(const DevImage& im) { return (uint64_t)im.wp * im.hp; }
+static uint64_t js_nblk(const DevImage& im) { return (uint64_t)im.blk_xmax * im.blk_ymax; }
+#define JS_OUT(f, hf, elem, chroma, off, count, total) { offsetof(DevBatch, f), offsetof(jsgpu_host_outputs, hf), elem, chroma, off, count, &BatchPlan::total }
+static const JsOutput js_outputs[] = {
+    JS_OUT(pix_y,   pix_y,     2, false, &DevImage::pix_off, js_npx, pix),
+    JS_OUT(pix_cb,  pix_cb,    2, true,  &DevImage::pix_off, js_npx, pix),
+    JS_OUT(pix_cr,  pix_cr,    2, true,  &DevImage::pix_off, js_npx, pix),
+    JS_OUT(dib,     dib,       1, false, &DevImage::dib_off, [](const DevImage& im) { return js_npx(im) * 4; }, dib),
+    JS_OUT(blk_y,   blk_y,     2, false, &DevImage::blk_off, js_nblk, blk),
+    JS_OUT(blk_cb,  blk_cb,    2, true,  &DevImage::blk_off, js_nblk, blk),
+    JS_OUT(blk_cr,  blk_cr,    2, true,  &DevImage::blk_off, js_nblk, blk),
+    JS_OUT(mcu_map, mcu_map,   4, false, &DevImage::mcu_off, [](const DevImage& im) -> uint64_t { return im.nmcu; }, mcu),
+    JS_OUT(histo,   dht_histo, 4, false, nullptr, [](const DevImage&) -> uint64_t { return JSGPU_HISTO_WORDS; }, histo),
+    JS_OUT(stats,   stats,     4, false, nullptr, [](const DevImage&) -> uint64_t { return JSGPU_STAT_WORDS; }, stats),
+};
+#undef JS_OUT
+static_assert(sizeof js_outputs / sizeof js_outputs[0] == JSGPU_OUT_STATS + 1, "one entry per JSGPU_OUT_* selector");
+static_assert(offsetof(jsgpu_pools, stats) == offsetof(jsgpu_host_outputs, stats), "the ten outputs lead both structs");
+static uint64_t out_off(const JsOutput& o, const DevImage& im, uint32_t i) { return o.off ? im.*o.off : i * o.count(im); }
+static void* get_ptr(const void* s, size_t off) { void* p; memcpy(&p, (const uint8_t*)s + off, sizeof p); return p; }
+static void set_ptr(void* s, size_t off, void* p) { memcpy((uint8_t*)s + off, &p, sizeof p); }
 
 static bool preview_is_default(const jsgpu_preview& p)
 {
@@ -94,11 +163,11 @@ static bool preview_is_default(const jsgpu_preview& p)
 }
 static int run_preview(jsgpu_ctx* ctx, const jsgpu_preview& pv, int* launches)
 {
-    const size_t n = ctx->himg.size();
+    const size_t n = ctx->plan.img.size();
     CK(ctx->d_cstats.reserve(n * sizeof(jsgpu_colour_stats)));
-    CK(ctx->d_rowclip.reserve((size_t)ctx->rows_total * 4 + 16));
-    *launches += js_launch_preview(ctx->batch, pv, (jsgpu_colour_stats*)ctx->d_cstats.p, (uint32_t*)ctx->d_rowclip.p, ctx->rows_total,
-                                   ctx->max_hp, ctx->sm_count, ctx->stream);
+    CK(ctx->d_rowclip.reserve((size_t)ctx->plan.rows * 4 + 16));
+    *launches += js_launch_preview(ctx->batch, pv, (jsgpu_colour_stats*)ctx->d_cstats.p, (uint32_t*)ctx->d_rowclip.p, ctx->plan.rows,
+                                   ctx->plan.max_hp, ctx->sm_count, ctx->stream);
     ctx->pv_done = true;
     return JSGPU_OK;
 }
@@ -156,9 +225,6 @@ void jsgpu_free(jsgpu_ctx* ctx)
     js_search_free(ctx->search);
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    DevBuf* bufs[] = { &ctx->d_ctab, &ctx->d_li, &ctx->d_lf, &ctx->d_sym, &ctx->d_tables, &ctx->d_img, &ctx->d_items, &ctx->d_litems, &ctx->d_tiles, &ctx->d_ubits, &ctx->d_seg64, &ctx->d_ph, &ctx->d_rowtab, &ctx->d_ex, &ctx->d_cstats, &ctx->d_rowclip, &ctx->d_dt_ev, &ctx->d_dt_mat, &ctx->d_dt_scratch, &ctx->d_mc, &ctx->d_bits, &ctx->d_seg,
-                       &ctx->d_coef, &ctx->d_mcubits, &ctx->d_pix, &ctx->d_dib, &ctx->d_blk, &ctx->d_mcumap, &ctx->d_histo, &ctx->d_stats, &ctx->d_misc };
-    for (auto* b : bufs) b->release();
     for (auto& ev : ctx->ev) if (ev) cudaEventDestroy(ev);
     for (auto& ev : ctx->tev) if (ev) cudaEventDestroy(ev);
     for (auto& ev : ctx->evx) if (ev) cudaEventDestroy(ev);
@@ -297,7 +363,6 @@ int jsgpu_bcast_tables(jsgpu_ctx* ctx, jsgpu_tables* sets, uint32_t nsets, void*
     if (e == cudaSuccess) nr = bcast(tmp.p, tmp.p, bytes, 0 /* ncclChar */, root, nccl_comm, ctx->stream);
     if (e == cudaSuccess && nr == 0) e = cudaMemcpyAsync(sets, tmp.p, bytes, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess && nr == 0) e = cudaStreamSynchronize(ctx->stream);
-    tmp.release();
     if (nr != 0) return fail(ctx, JSGPU_ECUDA, "ncclBroadcast failed (ncclResult %d)", nr);
     if (e != cudaSuccess) return fail(ctx, JSGPU_ECUDA, "table broadcast failed: %s", cudaGetErrorString(e));
     return JSGPU_OK;
@@ -363,191 +428,196 @@ static bool plan_image(const jsgpu_image_desc& d, uint32_t nsets, DevImage& im)
     return true;
 }
 
-int jsgpu_batch_begin(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32_t n, uint64_t bitstream_bytes)
+// The plan of a batch: validation, every image's geometry and pool offsets, the work lists, the IDCT tiles, the marker-scan
+// chunks and the totals, on the host.  Images plan_image refuses are skipped: status 0x80000000, no pool space.
+static int plan_batch(const jsgpu_image_desc* imgs, uint32_t n, uint32_t nsets, uint64_t bitstream_bytes, BatchPlan& p, std::string& err)
 {
-    if (!ctx || !imgs || n == 0) return JSGPU_EINVAL;
-    if (!ctx->have_idct) return fail(ctx, JSGPU_ESTATE, "jsgpu_set_idct_tables() has not been called");
-    if (ctx->nsets == 0) return fail(ctx, JSGPU_ESTATE, "jsgpu_upload_tables() has not been called");
-    cudaSetDevice(ctx->device);
-    ctx->planned = false; ctx->decoded = false;
-    ctx->himg.assign(n, DevImage());
-    ctx->layout.assign(n, jsgpu_image_layout());
-    uint64_t pix = 0, dib = 0, blk = 0, mcu = 0, rows = 0, max_scan = 0, ub = 0;
-    uint32_t seg = 0, n_std = 0, n_nonstd = 0, plane_bytes = 0, seg_np = 0, n_psync = 0;
-    uint64_t pht = 0, rtt = 0, cst = 0; uint32_t max_cs = 0;
-    uint64_t rowt = 0; uint32_t max_hp = 0;
-    std::vector<uint32_t> mc_img;              // image of every 4096-byte chunk (marker scan)
-    std::vector<uint2> items, litems, items_np, litems_np, vitems;
-    std::vector<uint4> tiles, tcls[3];
+    p = BatchPlan();
+    p.img.assign(n, DevImage());
+    p.layout.assign(n, jsgpu_image_layout());
+    p.bits_len = bitstream_bytes;
+    std::vector<uint2> items_np, litems_np, vitems;
+    std::vector<uint4> tcls[3];
     for (uint32_t i = 0; i < n; i++) {
-        DevImage& im = ctx->himg[i];
-        jsgpu_image_layout& lo = ctx->layout[i];
-        memset(&lo, 0, sizeof lo);
-        bool ok = plan_image(imgs[i], ctx->nsets, im);
+        DevImage& im = p.img[i];
+        jsgpu_image_layout& lo = p.layout[i];
+        bool ok = plan_image(imgs[i], nsets, im);
         if (ok && (imgs[i].scan_offset > bitstream_bytes || imgs[i].scan_length > bitstream_bytes - imgs[i].scan_offset))
-            return fail(ctx, JSGPU_EINVAL, "image %u: scan [%llu,+%llu) outside the %llu-byte bitstream", i,
+            return fail(err, JSGPU_EINVAL, "image %u: scan [%llu,+%llu) outside the %llu-byte bitstream", i,
                         (unsigned long long)imgs[i].scan_offset, (unsigned long long)imgs[i].scan_length, (unsigned long long)bitstream_bytes);
-        if (ok && imgs[i].scan_length >= 0x1ffffff0ull) return fail(ctx, JSGPU_EINVAL, "image %u: scan longer than 512 MiB (bit positions are 32-bit)", i);
-        if (ok && (imgs[i].scan_offset & 15)) return fail(ctx, JSGPU_EINVAL, "image %u: scan_offset %llu is not 16-byte aligned (jsgpu_image_desc)", i, (unsigned long long)imgs[i].scan_offset);
+        if (ok && imgs[i].scan_length >= 0x1ffffff0ull) return fail(err, JSGPU_EINVAL, "image %u: scan longer than 512 MiB (bit positions are 32-bit)", i);
+        if (ok && (imgs[i].scan_offset & 15)) return fail(err, JSGPU_EINVAL, "image %u: scan_offset %llu is not 16-byte aligned (jsgpu_image_desc)", i, (unsigned long long)imgs[i].scan_offset);
         if (!ok) {            // skipped image: no pool space, but keep seg_first monotone (k_finalize_mcumap binary-searches it)
-            im.valid = 0; im.nseg = 0; im.seg_first = seg; lo.status = 0x80000000u; continue;
+            im.valid = 0; im.nseg = 0; im.seg_first = p.nseg; lo.status = 0x80000000u; continue;
         }
-        im.pix_off = pix; im.dib_off = dib; im.blk_off = blk; im.mcu_off = mcu; im.seg_first = seg;
-        for (uint32_t c = 0; c < im.ns; c++) { im.coef_row[c] = rows; rows += (uint64_t)im.cw[c] * im.ch[c]; }
+        im.pix_off = p.pix; im.dib_off = p.dib; im.blk_off = p.blk; im.mcu_off = p.mcu; im.seg_first = p.nseg;
+        for (uint32_t c = 0; c < im.ns; c++) { im.coef_row[c] = p.coef_rows; p.coef_rows += (uint64_t)im.cw[c] * im.ch[c]; }
         uint64_t npx = (uint64_t)im.wp * im.hp;
-        im.row_off = rowt; rowt += im.hp; max_hp = std::max(max_hp, im.hp);
-        im.mc_first = mc_img.size(); im.mc_n = (uint32_t)((im.scan_len + 4095) >> 12); if (im.mc_n == 0) im.mc_n = 1;
-        mc_img.insert(mc_img.end(), im.mc_n, i);
-        pix += align_up(npx, 64); dib += align_up(npx * 4, 256); blk += align_up((uint64_t)im.blk_xmax * im.blk_ymax, 64);
-        mcu += align_up(im.nmcu, 32); seg += im.nseg;
-        max_scan = std::max(max_scan, im.scan_len);
-        for (uint32_t k = 0; k < im.nseg; k += JS_HUFF_WARPS) items.push_back(make_uint2(i, k));
-        for (uint32_t k = 0; k < im.nseg; k += JS_LANE_SEGS) litems.push_back(make_uint2(i, k));
+        im.row_off = p.rows; p.rows += im.hp; p.max_hp = std::max(p.max_hp, im.hp);
+        im.mc_first = p.mc_img.size(); im.mc_n = (uint32_t)((im.scan_len + 4095) >> 12); if (im.mc_n == 0) im.mc_n = 1;
+        p.mc_img.insert(p.mc_img.end(), im.mc_n, i);
+        p.pix += align_up(npx, 64); p.dib += align_up(npx * 4, 256); p.blk += align_up((uint64_t)im.blk_xmax * im.blk_ymax, 64);
+        p.mcu += align_up(im.nmcu, 32); p.nseg += im.nseg;
+        p.max_scan_len = std::max(p.max_scan_len, im.scan_len);
+        for (uint32_t k = 0; k < im.nseg; k += JS_HUFF_WARPS) p.items.push_back(make_uint2(i, k));
+        for (uint32_t k = 0; k < im.nseg; k += JS_LANE_SEGS) p.litems.push_back(make_uint2(i, k));
         const uint64_t uregion = align_up(im.scan_len + (uint64_t)JS_USLACK * im.nseg + 128, 256);
-        im.ubits_off = ub; ub += uregion;
+        im.ubits_off = p.ubits; p.ubits += uregion;
         if (im.psync) {           // slots of the self-synchronising passes + row table of k_unstuff
-            n_psync++;
-            im.ph_nslots = (uint32_t)(uregion >> 9) + im.nseg + 2; im.ph_first = pht; pht += (uint64_t)im.ph_nslots + 1;
-            im.rt_off = rtt; rtt += (im.scan_len >> 7) + 2ull * im.nseg + 4;
-            im.cs_nslots = (uint32_t)(im.scan_len >> 12) + 2 * im.nseg + 2; im.cs_first = cst; cst += im.cs_nslots; max_cs = std::max(max_cs, im.cs_nslots);
+            p.n_psync++;
+            im.ph_nslots = (uint32_t)(uregion >> 9) + im.nseg + 2; im.ph_first = p.ph; p.ph += (uint64_t)im.ph_nslots + 1;
+            im.rt_off = p.rt; p.rt += (im.scan_len >> 7) + 2ull * im.nseg + 4;
+            im.cs_nslots = (uint32_t)(im.scan_len >> 12) + 2 * im.nseg + 2; im.cs_first = p.cs; p.cs += im.cs_nslots; p.max_cs = std::max(p.max_cs, im.cs_nslots);
             for (uint32_t k = 0; k < im.ph_nslots; k += JS_LANE_SEGS) vitems.push_back(make_uint2(i, k));
         } else {
-            seg_np += im.nseg;
+            p.nseg_np += im.nseg;
             for (uint32_t k = 0; k < im.nseg; k += JS_HUFF_WARPS) items_np.push_back(make_uint2(i, k));
             for (uint32_t k = 0; k < im.nseg; k += JS_LANE_SEGS) litems_np.push_back(make_uint2(i, k));
         }
         if (im.std_layout) {
-            n_std++;
+            p.n_std++;
             const uint32_t ehc = (im.ns == 3) ? im.eh[1] : 1, cls = (ehc == 1) ? 0 : (ehc == 2) ? 1 : 2;
             for (uint32_t r = 0; r < im.mcu_ymax; r++) for (uint32_t t = 0; t < im.tiles_per_row; t++) {
                 uint32_t c0 = t * im.tile_mcus;
                 tcls[cls].push_back(make_uint4(i, r, c0, std::min(im.tile_mcus, im.mcu_xmax - c0)));
             }
             uint32_t bpt = 0; for (uint32_t c = 0; c < im.ns; c++) bpt += im.H[c] * im.V[c] * im.tile_mcus;
-            plane_bytes = std::max(plane_bytes, bpt * 128);
-        } else n_nonstd++;
+            p.plane_bytes = std::max(p.plane_bytes, bpt * 128);
+        } else p.n_nonstd++;
         lo.mcu_w = im.mcu_w; lo.mcu_h = im.mcu_h; lo.mcu_xmax = im.mcu_xmax; lo.mcu_ymax = im.mcu_ymax;
         lo.blk_xmax = im.blk_xmax; lo.blk_ymax = im.blk_ymax; lo.img_x = im.wp; lo.img_y = im.hp;
         lo.num_segments = im.nseg; lo.pix_off = im.pix_off; lo.dib_off = im.dib_off; lo.blk_off = im.blk_off; lo.mcu_off = im.mcu_off;
     }
-    uint32_t tcls_first[3], tcls_count[3];
-    for (int k = 0; k < 3; k++) { tcls_first[k] = (uint32_t)tiles.size(); tcls_count[k] = (uint32_t)tcls[k].size(); tiles.insert(tiles.end(), tcls[k].begin(), tcls[k].end()); }
-    ctx->bits_len = bitstream_bytes; ctx->pix_total = pix; ctx->dib_total = dib; ctx->blk_total = blk; ctx->mcu_total = mcu;
-    ctx->coef_rows = rows; ctx->max_scan_len = max_scan; ctx->ubits_total = ub; ctx->n_std = n_std; ctx->n_nonstd = n_nonstd;
-    ctx->ph_total = pht; ctx->rt_total = rtt; ctx->nseg_np = seg_np; ctx->n_psync = n_psync; ctx->max_cs = max_cs; ctx->cs_total = cst;
-    ctx->host_delivered = false; ctx->layout_only = ctx->plan_only;
-    if (ctx->plan_only) { ctx->planned = true; return JSGPU_OK; }
-    // allocate
-    CK(ctx->d_img.reserve(sizeof(DevImage) * (size_t)n));
-    CK(ctx->d_items.reserve(sizeof(uint2) * std::max<size_t>(items.size() + items_np.size(), 1)));
-    CK(ctx->d_bits.reserve(bitstream_bytes + 64));
-    CK(ctx->d_ubits.reserve(ub + 16384));          // + slack: a reader of corrupt data stops at the next MCU boundary, at most one MCU (<= 12 KB of bits) past the end
-    CK(ctx->d_litems.reserve(sizeof(uint2) * std::max<size_t>(litems.size() + litems_np.size() + vitems.size(), 1)));
-    CK(ctx->d_ph.reserve(pht * 72 + (size_t)n * 8 + 256));      // x 8 + ver 4 + k 4 + cnt 16 + aux 16 + pre 16 + two work lists 8 bytes per slot; two list lengths per image
-    CK(ctx->d_rowtab.reserve(rtt * 20 + cst * 12 + 256));       // rowtab 4 + rowmask 16 bytes per 128-byte raw row; 3 words per 4 KB chunk
-    CK(ctx->d_tiles.reserve(sizeof(uint4) * std::max<size_t>(tiles.size(), 1)));
-    CK(ctx->d_seg64.reserve(8 * (size_t)seg + 16));
-    CK(ctx->d_seg.reserve(sizeof(uint32_t) * ((7 + JS_STUFF_LIST) * (size_t)seg + 2 * (size_t)n + 16)));
-    CK(ctx->d_coef.reserve(rows * 128 + 4096));      // + 4096 spare bytes: no kernel addresses them (every row index is bounded by
-                                                     // its plane); kept so that the pool sizes stay as measured
-    CK(ctx->d_mcubits.reserve(mcu * 4 + 16));
-    CK(ctx->d_pix.reserve(pix * 2 * 3 + 64));
-    CK(ctx->d_dib.reserve(dib + 64));
-    CK(ctx->d_blk.reserve(blk * 2 * 3 + 64));
-    CK(ctx->d_mcumap.reserve(mcu * 4 + 16));
-    CK(ctx->d_histo.reserve((size_t)n * 2 * 4 * 17 * 4));
-    CK(ctx->d_stats.reserve((size_t)n * 16 * 4));
-    CK(ctx->d_misc.reserve((size_t)n * (8 + 8 + 4 + 4) + 64 + 64));
-    CK(ctx->d_ex.reserve((size_t)n * sizeof(JsExResult)));
-    ctx->rows_total = rowt; ctx->max_hp = max_hp; ctx->pv_done = false;
-    CK(ctx->d_mc.reserve(mc_img.size() * 4 + (mc_img.size() + 2) * 8 + 64));
-    if (!mc_img.empty()) CK(cudaMemcpyAsync(ctx->d_mc.p, mc_img.data(), mc_img.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-    ctx->mc_total = (uint32_t)mc_img.size();
-    CK(cudaMemcpyAsync(ctx->d_img.p, ctx->himg.data(), sizeof(DevImage) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-    const size_t n_it = items.size(), n_lit = litems.size();
-    items.insert(items.end(), items_np.begin(), items_np.end());                   // [all | without self-synchronised images]
-    litems.insert(litems.end(), litems_np.begin(), litems_np.end());               // [all | without ... | slots of the self-synchronised images]
-    litems.insert(litems.end(), vitems.begin(), vitems.end());
-    if (!items.empty()) CK(cudaMemcpyAsync(ctx->d_items.p, items.data(), sizeof(uint2) * items.size(), cudaMemcpyHostToDevice, ctx->stream));
-    if (!litems.empty()) CK(cudaMemcpyAsync(ctx->d_litems.p, litems.data(), sizeof(uint2) * litems.size(), cudaMemcpyHostToDevice, ctx->stream));
-    if (!tiles.empty()) CK(cudaMemcpyAsync(ctx->d_tiles.p, tiles.data(), sizeof(uint4) * tiles.size(), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));      // the work lists are locals
+    p.histo = (uint64_t)n * JSGPU_HISTO_WORDS; p.stats = (uint64_t)n * JSGPU_STAT_WORDS;
+    p.n_items = (uint32_t)p.items.size(); p.n_items_np = (uint32_t)items_np.size();
+    p.items.insert(p.items.end(), items_np.begin(), items_np.end());
+    p.n_litems = (uint32_t)p.litems.size(); p.n_litems_np = (uint32_t)litems_np.size(); p.n_vitems = (uint32_t)vitems.size();
+    p.litems.insert(p.litems.end(), litems_np.begin(), litems_np.end());
+    p.litems.insert(p.litems.end(), vitems.begin(), vitems.end());
+    for (int k = 0; k < 3; k++) { p.tcls_first[k] = (uint32_t)p.tiles.size(); p.tcls_count[k] = (uint32_t)tcls[k].size(); p.tiles.insert(p.tiles.end(), tcls[k].begin(), tcls[k].end()); }
+    return JSGPU_OK;
+}
+
+// A new batch: the context holds none until its plan (and, for jsgpu_batch_begin, its pools) is complete
+static int begin_plan(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32_t n, uint64_t bitstream_bytes)
+{
+    if (!ctx->have_idct) return fail(ctx, JSGPU_ESTATE, "jsgpu_set_idct_tables() has not been called");
+    if (ctx->nsets == 0) return fail(ctx, JSGPU_ESTATE, "jsgpu_upload_tables() has not been called");
+    cudaSetDevice(ctx->device);
+    ctx->state = JS_NO_BATCH;
+    return plan_batch(imgs, n, ctx->nsets, bitstream_bytes, ctx->plan, ctx->err);
+}
+
+int jsgpu_batch_begin(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32_t n, uint64_t bitstream_bytes)
+{
+    if (!ctx || !imgs || n == 0) return JSGPU_EINVAL;
+    const int r = begin_plan(ctx, imgs, n, bitstream_bytes); if (r) return r;
+    const BatchPlan& p = ctx->plan;
     DevBatch& b = ctx->batch;
     memset(&b, 0, sizeof b);
+    // allocate; carve() sizes the sub-allocated pools from their layouts and binds them
+    CK(ctx->d_img.reserve(sizeof(DevImage) * (size_t)n));
+    CK(ctx->d_items.reserve(sizeof(uint2) * std::max<size_t>(p.items.size(), 1)));
+    CK(ctx->d_bits.reserve(bitstream_bytes + 64));
+    CK(ctx->d_ubits.reserve(p.ubits + 16384));     // + slack: a reader of corrupt data stops at the next MCU boundary, at most one MCU (<= 12 KB of bits) past the end
+    CK(ctx->d_litems.reserve(sizeof(uint2) * std::max<size_t>(p.litems.size(), 1)));
+    auto ph = [&](Carve& c) {       // slot arrays, 16-byte members first; two list lengths per image
+        c.take(b.ph_cnt, p.ph); c.take(b.ph_aux, p.ph); c.take(b.ph_pre, p.ph); c.take(b.ph_x, p.ph);
+        c.take(b.ph_ver, p.ph); c.take(b.ph_k, p.ph); c.take(b.ph_list[0], p.ph); c.take(b.ph_list[1], p.ph);
+        c.take(b.ph_nl[0], n); c.take(b.ph_nl[1], n); c.skip(256);
+    };
+    CK(carve(ctx->d_ph, ph));
+    auto rowtab = [&](Carve& c) {   // per 128-byte raw row: row mask, unstuffed bytes before it; per 4 KB chunk: three words
+        c.take(b.rowmask, p.rt); c.take(b.rowtab, p.rt); c.take(b.cs_cnt, p.cs); c.take(b.cs_off, p.cs); c.take(b.cs_seg, p.cs); c.skip(256);
+    };
+    CK(carve(ctx->d_rowtab, rowtab));
+    CK(ctx->d_tiles.reserve(sizeof(uint4) * std::max<size_t>(p.tiles.size(), 1)));
+    CK(ctx->d_seg64.reserve(8 * (size_t)p.nseg + 16));
+    auto seg = [&](Carve& c) {
+        c.take(b.seg_start, p.nseg); c.take(b.seg_end, p.nseg); c.take(b.seg_endbits, p.nseg); c.take(b.seg_status, p.nseg);
+        c.take(b.seg_ulen, p.nseg); c.take(b.scan_end, n); c.take(b.nseg_found, n); c.take(b.seg_nstuff, p.nseg);
+        c.take(b.seg_stuff, (uint64_t)JS_STUFF_LIST * p.nseg); c.take(b.ovf_list, p.nseg); c.skip(64);
+    };
+    CK(carve(ctx->d_seg, seg));
+    CK(ctx->d_coef.reserve(p.coef_rows * 128 + 4096));    // + 4096 spare bytes: no kernel addresses them (every row index is bounded by
+                                                           // its plane); kept so that the pool sizes stay as measured
+    CK(ctx->d_mcubits.reserve(p.mcu * 4 + 16));
+    auto pix = [&](Carve& c) { c.take(b.pix_y, p.pix); c.take(b.pix_cb, p.pix); c.take(b.pix_cr, p.pix); c.skip(64); };
+    CK(carve(ctx->d_pix, pix));
+    CK(ctx->d_dib.reserve(p.dib + 64));
+    auto blk = [&](Carve& c) { c.take(b.blk_y, p.blk); c.take(b.blk_cb, p.blk); c.take(b.blk_cr, p.blk); c.skip(64); };
+    CK(carve(ctx->d_blk, blk));
+    CK(ctx->d_mcumap.reserve(p.mcu * 4 + 16));
+    CK(ctx->d_histo.reserve(p.histo * 4));
+    CK(ctx->d_stats.reserve(p.stats * 4));
+    static_assert(1 + PH_MAX_ROUNDS + 2 <= 16, "ovf_count and ph_nchg share one 64-byte block");
+    auto misc = [&](Carve& c) {     // per image: brightest-pixel key, luma sum, status word; the counters; per image: exact-path flag
+        c.take(b.bright_key, n); c.take(b.sum_y, n); c.take(b.img_status, n);
+        c.take(b.ovf_count, 1); c.take(b.ph_nchg, 15); c.take(b.ex_flag, n); c.skip(64);
+    };
+    CK(carve(ctx->d_misc, misc));
+    CK(ctx->d_ex.reserve((size_t)n * sizeof(JsExResult)));
+    auto mc = [&](Carve& c) { c.take(b.mc_img, p.mc_img.size()); c.align(64); c.take(b.mc_state, p.mc_img.size() + 2); };
+    CK(carve(ctx->d_mc, mc));
+    ctx->pv_done = false;
+    if (!p.mc_img.empty()) CK(cudaMemcpyAsync(b.mc_img, p.mc_img.data(), p.mc_img.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_img.p, p.img.data(), sizeof(DevImage) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+    if (!p.items.empty()) CK(cudaMemcpyAsync(ctx->d_items.p, p.items.data(), sizeof(uint2) * p.items.size(), cudaMemcpyHostToDevice, ctx->stream));
+    if (!p.litems.empty()) CK(cudaMemcpyAsync(ctx->d_litems.p, p.litems.data(), sizeof(uint2) * p.litems.size(), cudaMemcpyHostToDevice, ctx->stream));
+    if (!p.tiles.empty()) CK(cudaMemcpyAsync(ctx->d_tiles.p, p.tiles.data(), sizeof(uint4) * p.tiles.size(), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));      // the next plan rewrites these host arrays
     b.img = (const DevImage*)ctx->d_img.p; b.tables = (const DevTableSet*)ctx->d_tables.p; b.nimg = n;
-    b.bits = (const uint8_t*)ctx->d_bits.p; b.bits_len = bitstream_bytes;
-    uint32_t* sp = (uint32_t*)ctx->d_seg.p;
-    b.seg_start = sp; b.seg_end = sp + seg; b.seg_endbits = sp + 2 * (size_t)seg; b.seg_status = sp + 3 * (size_t)seg;
-    b.seg_ulen = sp + 4 * (size_t)seg;
-    b.scan_end = sp + 5 * (size_t)seg; b.nseg_found = b.scan_end + n; b.nseg_total = seg;
-    b.seg_nstuff = b.nseg_found + n; b.seg_stuff = b.seg_nstuff + seg; b.ovf_list = b.seg_stuff + (size_t)JS_STUFF_LIST * seg;
+    b.bits = (const uint8_t*)ctx->d_bits.p; b.bits_len = bitstream_bytes; b.nseg_total = p.nseg;
     b.seg_uoff = (unsigned long long*)ctx->d_seg64.p; b.ubits = (uint8_t*)ctx->d_ubits.p;
-    b.litems = (const uint2*)ctx->d_litems.p; b.nlitems = (uint32_t)n_lit;
-    b.litems_np = b.litems + n_lit; b.nlitems_np = (uint32_t)litems_np.size();
-    b.vitems = b.litems_np + litems_np.size(); b.nvitems = (uint32_t)vitems.size();
-    {   // slot arrays, 16-byte members first
-        uint8_t* q = (uint8_t*)ctx->d_ph.p;
-        b.ph_cnt = (uint4*)q; q += pht * 16; b.ph_aux = (uint4*)q; q += pht * 16; b.ph_pre = (uint4*)q; q += pht * 16;
-        b.ph_x = (unsigned long long*)q; q += pht * 8; b.ph_ver = (uint32_t*)q; q += pht * 4; b.ph_k = (uint32_t*)q; q += pht * 4;
-        b.ph_list[0] = (uint32_t*)q; q += pht * 4; b.ph_list[1] = (uint32_t*)q; q += pht * 4;
-        b.ph_nl[0] = (uint32_t*)q; q += (size_t)n * 4; b.ph_nl[1] = (uint32_t*)q;
-        b.rowmask = (uint4*)ctx->d_rowtab.p; b.rowtab = (uint32_t*)((uint8_t*)ctx->d_rowtab.p + rtt * 16);
-        b.cs_cnt = b.rowtab + rtt; b.cs_off = b.cs_cnt + cst; b.cs_seg = b.cs_off + cst;
-    }
-    b.tiles = (const uint4*)ctx->d_tiles.p; b.ntiles = (uint32_t)tiles.size(); b.tile_plane_bytes = plane_bytes;
-    for (int k = 0; k < 3; k++) { b.tcls_first[k] = tcls_first[k]; b.tcls_count[k] = tcls_count[k]; }
-    b.items = (const uint2*)ctx->d_items.p; b.nitems = (uint32_t)n_it;
-    b.items_np = b.items + n_it; b.nitems_np = (uint32_t)items_np.size();
+    b.litems = (const uint2*)ctx->d_litems.p; b.nlitems = p.n_litems;
+    b.litems_np = b.litems + p.n_litems; b.nlitems_np = p.n_litems_np;
+    b.vitems = b.litems_np + p.n_litems_np; b.nvitems = p.n_vitems;
+    b.items = (const uint2*)ctx->d_items.p; b.nitems = p.n_items;
+    b.items_np = b.items + p.n_items; b.nitems_np = p.n_items_np;
+    b.tiles = (const uint4*)ctx->d_tiles.p; b.ntiles = (uint32_t)p.tiles.size(); b.tile_plane_bytes = p.plane_bytes;
+    for (int k = 0; k < 3; k++) { b.tcls_first[k] = p.tcls_first[k]; b.tcls_count[k] = p.tcls_count[k]; }
     b.coef = (int16_t*)ctx->d_coef.p; b.mcu_bitpos = (uint32_t*)ctx->d_mcubits.p;
-    b.pix_y = (int16_t*)ctx->d_pix.p; b.pix_cb = b.pix_y + pix; b.pix_cr = b.pix_cb + pix;
-    b.dib = (uint8_t*)ctx->d_dib.p;
-    b.blk_y = (int16_t*)ctx->d_blk.p; b.blk_cb = b.blk_y + blk; b.blk_cr = b.blk_cb + blk;
-    b.mcu_map = (uint32_t*)ctx->d_mcumap.p;
+    b.dib = (uint8_t*)ctx->d_dib.p; b.mcu_map = (uint32_t*)ctx->d_mcumap.p;
     b.histo = (uint32_t*)ctx->d_histo.p; b.stats = (int32_t*)ctx->d_stats.p;
-    b.mc_img = (uint32_t*)ctx->d_mc.p; b.mc_total = ctx->mc_total;
-    b.mc_state = (unsigned long long*)((uint8_t*)ctx->d_mc.p + (((size_t)ctx->mc_total * 4 + 63) & ~(size_t)63));
-    b.bright_key = (unsigned long long*)ctx->d_misc.p; b.sum_y = b.bright_key + n; b.img_status = (uint32_t*)(b.sum_y + n); b.ovf_count = b.img_status + n;
-    b.ph_nchg = b.ovf_count + 1; b.ex_flag = b.ph_nchg + PH_MAX_ROUNDS + 2; b.ex_res = (JsExResult*)ctx->d_ex.p;
-    ctx->planned = true;
+    b.mc_total = (uint32_t)p.mc_img.size(); b.ex_res = (JsExResult*)ctx->d_ex.p;
+    ctx->state = JS_PLANNED;
     return JSGPU_OK;
 }
 
 int jsgpu_batch_layout(jsgpu_ctx* ctx, jsgpu_image_layout* out, uint32_t n)
 {
     if (!ctx || !out) return JSGPU_EINVAL;
-    if (!ctx->planned) return fail(ctx, JSGPU_ESTATE, "no batch planned");
-    if (n > ctx->layout.size()) n = (uint32_t)ctx->layout.size();
-    if (ctx->decoded && !ctx->host_delivered) {
+    if (ctx->state == JS_NO_BATCH) return fail(ctx, JSGPU_ESTATE, "no batch planned");
+    std::vector<jsgpu_image_layout>& layout = ctx->plan.layout;
+    if (n > layout.size()) n = (uint32_t)layout.size();
+    if (ctx->state == JS_DECODED) {
         cudaSetDevice(ctx->device);
-        std::vector<uint32_t> st(ctx->layout.size());
+        std::vector<uint32_t> st(layout.size());
         CK(cudaMemcpyAsync(st.data(), ctx->batch.img_status, st.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        std::vector<uint32_t> ex(ctx->layout.size());
+        std::vector<uint32_t> ex(layout.size());
         CK(cudaMemcpyAsync(ex.data(), ctx->batch.ex_flag, ex.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        for (size_t i = 0; i < st.size(); i++) if (ctx->himg[i].valid) ctx->layout[i].status = st[i] | (ex[i] ? JSGPU_ST_EXACT : 0u);
+        for (size_t i = 0; i < st.size(); i++) if (ctx->plan.img[i].valid) layout[i].status = st[i] | (ex[i] ? JSGPU_ST_EXACT : 0u);
     }
-    memcpy(out, ctx->layout.data(), sizeof(jsgpu_image_layout) * n);
+    memcpy(out, layout.data(), sizeof(jsgpu_image_layout) * n);
     return JSGPU_OK;
 }
 
 int jsgpu_batch_pools(jsgpu_ctx* ctx, jsgpu_pools* out)
 {
     if (!ctx || !out) return JSGPU_EINVAL;
-    if (!ctx->planned) return fail(ctx, JSGPU_ESTATE, "no batch planned");
-    if (ctx->host_delivered) return fail(ctx, JSGPU_ESTATE, "the last batch was delivered to host buffers by jsgpu_decode_batch_host");
-    const DevBatch& b = ctx->batch;
-    out->pix_y = b.pix_y; out->pix_cb = b.pix_cb; out->pix_cr = b.pix_cr; out->dib = b.dib;
-    out->blk_y = b.blk_y; out->blk_cb = b.blk_cb; out->blk_cr = b.blk_cr; out->mcu_map = b.mcu_map;
-    out->dht_histo = b.histo; out->stats = b.stats; out->coef = b.coef; out->bitstream = (uint8_t*)ctx->d_bits.p;
+    if (ctx->state < JS_PLANNED) return fail(ctx, JSGPU_ESTATE, "%s", ctx->state == JS_LAYOUT_ONLY ? HOST_DELIVERED : "no batch planned");
+    for (const JsOutput& o : js_outputs) set_ptr(out, o.host, get_ptr(&ctx->batch, o.dev));
+    out->coef = ctx->batch.coef; out->bitstream = (uint8_t*)ctx->d_bits.p;
     return JSGPU_OK;
 }
 
 int jsgpu_batch_upload(jsgpu_ctx* ctx, const uint8_t* host, uint64_t bytes)
 {
     if (!ctx || !host) return JSGPU_EINVAL;
-    if (!ctx->planned || ctx->layout_only) return fail(ctx, JSGPU_ESTATE, "no batch planned");
-    if (bytes > ctx->bits_len) return fail(ctx, JSGPU_EINVAL, "upload larger than the planned bitstream");
+    if (ctx->state < JS_PLANNED) return fail(ctx, JSGPU_ESTATE, "no batch planned");
+    if (bytes > ctx->plan.bits_len) return fail(ctx, JSGPU_EINVAL, "upload larger than the planned bitstream");
     cudaSetDevice(ctx->device);
     CK(cudaMemcpyAsync(ctx->d_bits.p, host, bytes, cudaMemcpyHostToDevice, ctx->stream));
     return JSGPU_OK;
@@ -564,7 +634,7 @@ static int detail_prepare(jsgpu_ctx* ctx, int err_max, int* launches)
     const DevBatch& b = ctx->batch;
     cudaStream_t s = ctx->stream;
     const jsgpu_detail& dtl = ctx->dtl;
-    const DevImage& im = ctx->himg[dtl.image];
+    const DevImage& im = ctx->plan.img[dtl.image];
     // the walk decodes MCUs 0 .. end-1 and prints those from base on (its arithmetic: a 32-bit base, a 64-bit end)
     const uint32_t base = dtl.mcu_y * im.mcu_xmax + dtl.mcu_x;
     const uint32_t end = im.valid ? (uint32_t)std::min<unsigned long long>(im.nmcu, (unsigned long long)base + dtl.len) : 0u;
@@ -577,12 +647,12 @@ static int detail_prepare(jsgpu_ctx* ctx, int err_max, int* launches)
         CK(cudaMemcpyAsync(&status, b.img_status + dtl.image, 4, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
     }
-    CK(ctx->d_dt_scratch.reserve((16 + 136 + 2 * (size_t)r.n) * 4));
+    CK(ctx->d_dt_scratch.reserve((16 + JSGPU_HISTO_WORDS + 2 * (size_t)r.n) * 4));
     uint32_t* hdr = (uint32_t*)ctx->d_dt_scratch.p;
     CK(cudaMemsetAsync(hdr, 0, 16 * 4, s));
     uint64_t nev, nmat;
     if (status == 0) {
-        *launches += js_launch_detail_count(b, r, hdr + 16 + 136, hdr, err_max, s);
+        *launches += js_launch_detail_count(b, r, hdr + 16 + JSGPU_HISTO_WORDS, hdr, err_max, s);
         uint32_t tot[2];
         CK(cudaMemcpyAsync(tot, hdr, sizeof tot, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
@@ -603,14 +673,14 @@ static int detail_prepare(jsgpu_ctx* ctx, int err_max, int* launches)
 int jsgpu_batch_decode(jsgpu_ctx* ctx)
 {
     if (!ctx) return JSGPU_EINVAL;
-    if (!ctx->planned || ctx->layout_only) return fail(ctx, JSGPU_ESTATE, "no batch planned (the last jsgpu_decode_batch_host left only its layout here)");
+    if (ctx->state < JS_PLANNED) return fail(ctx, JSGPU_ESTATE, "no batch planned (the last jsgpu_decode_batch_host left only its layout here)");
     cudaSetDevice(ctx->device);
-    DevBatch& b = ctx->batch;
+    DevBatch& b = ctx->batch; const BatchPlan& p = ctx->plan;
     b.decode_ac = ctx->opt.decode_ac; b.want_histo = ctx->opt.want_histo; b.idct_mode = ctx->opt.idct_mode;
-    b.any_p12 = 0; for (const DevImage& im : ctx->himg) if (im.valid && im.precision > 8) b.any_p12 = 1;
+    b.any_p12 = 0; for (const DevImage& im : p.img) if (im.valid && im.precision > 8) b.any_p12 = 1;
     b.lane_nlut = 1; b.lane_l2_smem = 1; b.max_nseg = 0;
-    for (const DevImage& im : ctx->himg) if (im.valid) b.max_nseg = std::max(b.max_nseg, im.nseg);
-    for (const DevImage& im : ctx->himg) if (im.valid) {
+    for (const DevImage& im : p.img) if (im.valid) b.max_nseg = std::max(b.max_nseg, im.nseg);
+    for (const DevImage& im : p.img) if (im.valid) {
         uint32_t seen = 0, nl = 0;
         for (uint32_t c = 0; c < im.ns; c++) for (int cls = 0; cls < 2; cls++) {
             const uint32_t slot = cls ? im.slot_ac[c] : im.slot_dc[c];
@@ -622,19 +692,19 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx)
     int launches = 0;
     CK(cudaEventRecord(ctx->ev[0], s));
     // clear accumulators (the reference memsets its maps: ImgDecode.cpp:2900,2924-2928,2965)
-    CK(cudaMemsetAsync(b.histo, 0, (size_t)b.nimg * 2 * 4 * 17 * 4, s));
-    CK(cudaMemsetAsync(b.stats, 0, (size_t)b.nimg * 16 * 4, s));
+    CK(cudaMemsetAsync(b.histo, 0, p.histo * 4, s));
+    CK(cudaMemsetAsync(b.stats, 0, p.stats * 4, s));
     CK(cudaMemsetAsync(b.bright_key, 0, (size_t)b.nimg * (8 + 8 + 4) + 4, s));      // + ovf_count
-    CK(cudaMemsetAsync(b.mcu_map, 0, ctx->mcu_total * 4, s));
-    CK(cudaMemsetAsync(b.blk_y, 0, ctx->blk_total * 2 * 3, s));
+    CK(cudaMemsetAsync(b.mcu_map, 0, p.mcu * 4, s));
+    CK(cudaMemsetAsync(b.blk_y, 0, p.blk * 2 * 3, s));
     // exotic sampling layouts leave pixels of a component unwritten (a component with 1 < H < Hmax covers only part of the MCU): they
     // read as the 0 the reference's memset left there (ImgDecode.cpp:2924-2928); standard layouts write every pixel
-    if (ctx->n_nonstd) CK(cudaMemsetAsync(b.pix_y, 0, ctx->pix_total * 2 * 3, s));
-    launches += js_launch_marker_scan(b, ctx->max_scan_len, s);
+    if (p.n_nonstd) CK(cudaMemsetAsync(b.pix_y, 0, p.pix * 2 * 3, s));
+    launches += js_launch_marker_scan(b, p.max_scan_len, s);
     // long intervals: chunk-parallel unstuffing into the pre-zeroed pool (chunk edges are OR-ed in)
-    if (ctx->n_psync) CK(cudaMemsetAsync(ctx->d_ubits.p, 0, ctx->ubits_total + 16384, s));
-    if (ctx->n_psync < ctx->n_std + ctx->n_nonstd) launches += js_launch_unstuff(b, s);
-    if (ctx->n_psync) launches += js_launch_unstuff_long(b, ctx->max_cs, s);
+    if (p.n_psync) CK(cudaMemsetAsync(ctx->d_ubits.p, 0, p.ubits + 16384, s));
+    if (p.n_psync < p.n_std + p.n_nonstd) launches += js_launch_unstuff(b, s);
+    if (p.n_psync) launches += js_launch_unstuff_long(b, p.max_cs, s);
     CK(cudaEventRecord(ctx->ev[1], s));
     {
         // huff_kernel: 1 = one warp per restart interval for everything, 2 = one lane per restart interval for everything,
@@ -644,7 +714,7 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx)
         const bool selfsync = (hk == 0 || hk == 3) && b.nvitems > 0 && b.lane_l2_smem;
         DevBatch bh = b;
         uint32_t nseg_short = b.nseg_total;
-        if (selfsync) { bh.items = b.items_np; bh.nitems = b.nitems_np; bh.litems = b.litems_np; bh.nlitems = b.nlitems_np; nseg_short = ctx->nseg_np; }
+        if (selfsync) { bh.items = b.items_np; bh.nitems = b.nitems_np; bh.litems = b.litems_np; bh.nlitems = b.nlitems_np; nseg_short = p.nseg_np; }
         else bh.nvitems = 0;
         if (hk == 0 || hk == 3) hk = (nseg_short >= 4096) ? 2 : 1;       // many short intervals -> lane kernel
         if (hk == 2) launches += js_launch_huffman_lane(bh, ctx->sm_count, s);
@@ -675,7 +745,7 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx)
         CK(cudaStreamWaitEvent(ctx->stream2, ctx->evx[0], 0));
         launches += js_launch_finalize_maps(b, ctx->stream2);
         launches += js_launch_finalize_emptied(b, ctx->stream2);
-        if (ctx->dt_parallel) launches += js_launch_detail_emit(b, ctx->dt_range, (const uint32_t*)ctx->d_dt_scratch.p + 16 + 136, ctx->dt_out, ctx->stream2);
+        if (ctx->dt_parallel) launches += js_launch_detail_emit(b, ctx->dt_range, (const uint32_t*)ctx->d_dt_scratch.p + 16 + JSGPU_HISTO_WORDS, ctx->dt_out, ctx->stream2);
         CK(cudaEventRecord(ctx->evx[1], ctx->stream2));
         maps_forked = true;
     }
@@ -689,7 +759,7 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx)
         if (fused)
             launches += js_launch_idct_fused(b, (const IdctSym*)ctx->d_sym.p, (const ColorTabs*)ctx->d_ctab.p, ctx->sm_count,
                                              flt ? JS_TILE_FLOAT : ctx->tab_baked ? JS_TILE_INT_BAKED : JS_TILE_INT_SMEM, s);
-        if (!fused || ctx->n_nonstd > 0) {
+        if (!fused || p.n_nonstd > 0) {
             DevBatch bs = b; bs.simple_only_nonstd = fused ? 1 : 0;
             launches += js_launch_idct_simple(bs, (const int32_t*)ctx->d_li.p, (const float*)ctx->d_lf.p, s);
         }
@@ -706,7 +776,7 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx)
     CK(cudaEventRecord(ctx->ev[4], s));
     CK(cudaGetLastError());
     ctx->launches = launches;
-    ctx->decoded = true;
+    ctx->state = JS_DECODED;
     return JSGPU_OK;
 }
 
@@ -723,7 +793,7 @@ int jsgpu_batch_preview(jsgpu_ctx* ctx, const jsgpu_preview* p)
 {
     if (!ctx || !p) return JSGPU_EINVAL;
     if (p->mode < 0 || p->mode > 8) return fail(ctx, JSGPU_EINVAL, "preview mode must be 0..8 (snoop.h:100-108)");
-    if (!ctx->decoded || ctx->host_delivered) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to recolour");
+    if (ctx->state != JS_DECODED) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to recolour");
     cudaSetDevice(ctx->device);
     jsgpu_preview pv = *p; if (pv.mode == 0) pv.mode = 1;
     int launches = 0;
@@ -744,7 +814,7 @@ int jsgpu_set_detail(jsgpu_ctx* ctx, const jsgpu_detail* d)
 int jsgpu_batch_detail_info(jsgpu_ctx* ctx, uint32_t info[4])
 {
     if (!ctx || !info) return JSGPU_EINVAL;
-    if (!ctx->decoded || ctx->host_delivered || !ctx->dt_done) return fail(ctx, JSGPU_ESTATE, "the last decode collected no detailed decode (jsgpu_set_detail)");
+    if (ctx->state != JS_DECODED || !ctx->dt_done) return fail(ctx, JSGPU_ESTATE, "the last decode collected no detailed decode (jsgpu_set_detail)");
     cudaSetDevice(ctx->device);
     CK(cudaMemcpyAsync(info, ctx->dt_out.hdr, 2 * 4, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -795,9 +865,9 @@ int jsgpu_batch_export(jsgpu_ctx* ctx, uint32_t image, int mode, void* host_out,
 {
     if (!ctx || !host_out) return JSGPU_EINVAL;
     if (mode < JSGPU_EXPORT_RGB8 || mode > JSGPU_EXPORT_YCC8) return fail(ctx, JSGPU_EINVAL, "export mode must be 0 (RGB8), 1 (RGB16) or 2 (YCC8)");
-    if (!ctx->decoded || ctx->host_delivered) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to export");
-    if (image >= ctx->himg.size()) return fail(ctx, JSGPU_EINVAL, "image index out of range");
-    const DevImage& im = ctx->himg[image];
+    if (ctx->state != JS_DECODED) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to export");
+    if (image >= ctx->plan.img.size()) return fail(ctx, JSGPU_EINVAL, "image index out of range");
+    const DevImage& im = ctx->plan.img[image];
     if (!im.valid) return fail(ctx, JSGPU_EUNSUP, "image %u was skipped", image);
     if (mode == JSGPU_EXPORT_YCC8 && im.ns != 3) return fail(ctx, JSGPU_EUNSUP, "YCC export needs a three-component scan");
     const uint64_t npx = (uint64_t)im.wp * im.hp, need = npx * (mode == JSGPU_EXPORT_RGB16 ? 6 : 3);
@@ -809,7 +879,6 @@ int jsgpu_batch_export(jsgpu_ctx* ctx, uint32_t image, int mode, void* host_out,
     cudaError_t e = cudaMemcpyAsync(host_out, tmp.p, (size_t)need, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     if (e == cudaSuccess) e = cudaGetLastError();
-    tmp.release();
     if (e != cudaSuccess) return fail(ctx, JSGPU_ECUDA, "export failed: %s", cudaGetErrorString(e));
     return JSGPU_OK;
 }
@@ -817,8 +886,8 @@ int jsgpu_batch_export(jsgpu_ctx* ctx, uint32_t image, int mode, void* host_out,
 int jsgpu_batch_colour_stats(jsgpu_ctx* ctx, uint32_t image, jsgpu_colour_stats* out)
 {
     if (!ctx || !out) return JSGPU_EINVAL;
-    if (!ctx->decoded || ctx->host_delivered || !ctx->pv_done) return fail(ctx, JSGPU_ESTATE, "no preview pass has run on this batch (jsgpu_set_preview / jsgpu_batch_preview)");
-    if (image >= ctx->himg.size()) return fail(ctx, JSGPU_EINVAL, "image index out of range");
+    if (ctx->state != JS_DECODED || !ctx->pv_done) return fail(ctx, JSGPU_ESTATE, "no preview pass has run on this batch (jsgpu_set_preview / jsgpu_batch_preview)");
+    if (image >= ctx->plan.img.size()) return fail(ctx, JSGPU_EINVAL, "image index out of range");
     cudaSetDevice(ctx->device);
     CK(cudaMemcpyAsync(out, (const jsgpu_colour_stats*)ctx->d_cstats.p + image, sizeof *out, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -847,8 +916,8 @@ int jsgpu_batch_launches(jsgpu_ctx* ctx) { return ctx ? ctx->launches : JSGPU_EI
 int jsgpu_batch_errors(jsgpu_ctx* ctx, uint32_t image, jsgpu_scan_errors* out)
 {
     if (!ctx || !out) return JSGPU_EINVAL;
-    if (!ctx->decoded || ctx->host_delivered) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to report on");
-    if (image >= ctx->himg.size()) return fail(ctx, JSGPU_EINVAL, "image index out of range");
+    if (ctx->state != JS_DECODED) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to report on");
+    if (image >= ctx->plan.img.size()) return fail(ctx, JSGPU_EINVAL, "image index out of range");
     cudaSetDevice(ctx->device);
     uint32_t flag = 0;
     CK(cudaMemcpyAsync(&flag, ctx->batch.ex_flag + image, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -863,17 +932,16 @@ int jsgpu_batch_errors(jsgpu_ctx* ctx, uint32_t image, jsgpu_scan_errors* out)
 int jsgpu_batch_checksums(jsgpu_ctx* ctx, uint64_t* ck, uint32_t n)
 {
     if (!ctx || !ck) return JSGPU_EINVAL;
-    if (!ctx->decoded || ctx->host_delivered) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to checksum");
-    if (n > ctx->himg.size()) n = (uint32_t)ctx->himg.size();
+    if (ctx->state != JS_DECODED) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to checksum");
+    if (n > ctx->plan.img.size()) n = (uint32_t)ctx->plan.img.size();
     cudaSetDevice(ctx->device);
     static_assert(JSGPU_CK_WORDS == JSGPU_CK_WORDS_INTERNAL, "checksum layout");
     DevBuf tmp;
-    CK(tmp.reserve((size_t)ctx->himg.size() * JSGPU_CK_WORDS * 8));
+    CK(tmp.reserve((size_t)ctx->plan.img.size() * JSGPU_CK_WORDS * 8));
     js_launch_checksums(ctx->batch, (unsigned long long*)tmp.p, ctx->stream);
     cudaError_t e = cudaMemcpyAsync(ck, tmp.p, (size_t)n * JSGPU_CK_WORDS * 8, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     if (e == cudaSuccess) e = cudaGetLastError();
-    tmp.release();
     if (e != cudaSuccess) return fail(ctx, JSGPU_ECUDA, "checksum kernel failed: %s", cudaGetErrorString(e));
     return JSGPU_OK;
 }
@@ -881,12 +949,12 @@ int jsgpu_batch_checksums(jsgpu_ctx* ctx, uint64_t* ck, uint32_t n)
 int jsgpu_batch_selfsync_info(jsgpu_ctx* ctx, uint32_t* info, uint32_t n)
 {
     if (!ctx || !info || n < 4) return JSGPU_EINVAL;
-    if (!ctx->decoded || ctx->host_delivered) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to report on");
+    if (ctx->state != JS_DECODED) return fail(ctx, JSGPU_ESTATE, "no device-resident decode to report on");
     cudaSetDevice(ctx->device);
     memset(info, 0, sizeof(uint32_t) * n);
-    info[0] = ctx->n_psync; info[1] = (uint32_t)std::min<uint64_t>(ctx->ph_total, 0xffffffffu); info[2] = PH_MAX_ROUNDS;
+    info[0] = ctx->plan.n_psync; info[1] = (uint32_t)std::min<uint64_t>(ctx->plan.ph, 0xffffffffu); info[2] = PH_MAX_ROUNDS;
     uint32_t h[PH_MAX_ROUNDS + 2] = {};
-    if (ctx->n_psync) {
+    if (ctx->plan.n_psync) {
         CK(cudaMemcpyAsync(h, ctx->batch.ph_nchg, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
     }
@@ -897,7 +965,7 @@ int jsgpu_batch_selfsync_info(jsgpu_ctx* ctx, uint32_t* info, uint32_t n)
 int jsgpu_batch_stage_ms(jsgpu_ctx* ctx, float* ms5)
 {
     if (!ctx || !ms5) return JSGPU_EINVAL;
-    if (!ctx->decoded) return fail(ctx, JSGPU_ESTATE, "nothing decoded yet");
+    if (ctx->state != JS_DECODED) return fail(ctx, JSGPU_ESTATE, "nothing decoded yet");
     cudaSetDevice(ctx->device);
     CK(cudaEventSynchronize(ctx->ev[4]));
     for (int i = 0; i < 4; i++) CK(cudaEventElapsedTime(&ms5[i], ctx->ev[i], ctx->ev[i + 1]));
@@ -908,27 +976,15 @@ int jsgpu_batch_stage_ms(jsgpu_ctx* ctx, float* ms5)
 int jsgpu_batch_download(jsgpu_ctx* ctx, int which, uint32_t image, void* dst, uint64_t bytes)
 {
     if (!ctx || !dst) return JSGPU_EINVAL;
-    if (!ctx->decoded) return fail(ctx, JSGPU_ESTATE, "nothing decoded yet");
-    if (ctx->host_delivered) return fail(ctx, JSGPU_ESTATE, "the last batch was delivered to host buffers by jsgpu_decode_batch_host");
-    if (image >= ctx->himg.size()) return fail(ctx, JSGPU_EINVAL, "image index out of range");
+    if (ctx->state != JS_DECODED) return fail(ctx, JSGPU_ESTATE, "%s", ctx->state == JS_LAYOUT_ONLY ? HOST_DELIVERED : "nothing decoded yet");
+    if (image >= ctx->plan.img.size()) return fail(ctx, JSGPU_EINVAL, "image index out of range");
     cudaSetDevice(ctx->device);
-    const DevImage& im = ctx->himg[image]; const DevBatch& b = ctx->batch;
+    const DevImage& im = ctx->plan.img[image];
     if (!im.valid) return fail(ctx, JSGPU_EUNSUP, "image %u was not decoded", image);
-    const void* src = nullptr; uint64_t avail = 0;
-    uint64_t npx = (uint64_t)im.wp * im.hp, nblk = (uint64_t)im.blk_xmax * im.blk_ymax;
-    switch (which) {
-    case JSGPU_OUT_PIX_Y:  src = b.pix_y + im.pix_off; avail = npx * 2; break;
-    case JSGPU_OUT_PIX_CB: src = b.pix_cb + im.pix_off; avail = (im.ns == 3) ? npx * 2 : 0; break;
-    case JSGPU_OUT_PIX_CR: src = b.pix_cr + im.pix_off; avail = (im.ns == 3) ? npx * 2 : 0; break;
-    case JSGPU_OUT_DIB:    src = b.dib + im.dib_off; avail = npx * 4; break;
-    case JSGPU_OUT_BLK_Y:  src = b.blk_y + im.blk_off; avail = nblk * 2; break;
-    case JSGPU_OUT_BLK_CB: src = b.blk_cb + im.blk_off; avail = (im.ns == 3) ? nblk * 2 : 0; break;
-    case JSGPU_OUT_BLK_CR: src = b.blk_cr + im.blk_off; avail = (im.ns == 3) ? nblk * 2 : 0; break;
-    case JSGPU_OUT_MCU_MAP: src = b.mcu_map + im.mcu_off; avail = (uint64_t)im.nmcu * 4; break;
-    case JSGPU_OUT_HISTO:  src = b.histo + (size_t)image * 2 * 4 * 17; avail = 2 * 4 * 17 * 4; break;
-    case JSGPU_OUT_STATS:  src = b.stats + (size_t)image * 16; avail = 16 * 4; break;
-    default: return fail(ctx, JSGPU_EINVAL, "unknown output selector %d", which);
-    }
+    if (which < 0 || which > JSGPU_OUT_STATS) return fail(ctx, JSGPU_EINVAL, "unknown output selector %d", which);
+    const JsOutput& o = js_outputs[which];
+    const uint8_t* src = (const uint8_t*)get_ptr(&ctx->batch, o.dev) + out_off(o, im, image) * o.elem;
+    const uint64_t avail = (o.chroma && im.ns != 3) ? 0 : o.count(im) * o.elem;
     if (bytes > avail) return fail(ctx, JSGPU_EINVAL, "output %d of image %u has %llu bytes, %llu requested", which, image,
                                    (unsigned long long)avail, (unsigned long long)bytes);
     CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
@@ -943,31 +999,22 @@ static int decode_host_single(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint
     int r = jsgpu_batch_begin(ctx, imgs, n, bytes); if (r) return r;
     r = jsgpu_batch_upload(ctx, bits, bytes); if (r) return r;
     r = jsgpu_batch_decode(ctx); if (r) return r;
-    const DevBatch& b = ctx->batch; cudaStream_t s = ctx->stream;
-    if (out->pix_y)  CK(cudaMemcpyAsync(out->pix_y,  b.pix_y,  ctx->pix_total * 2, cudaMemcpyDeviceToHost, s));
-    if (out->pix_cb) CK(cudaMemcpyAsync(out->pix_cb, b.pix_cb, ctx->pix_total * 2, cudaMemcpyDeviceToHost, s));
-    if (out->pix_cr) CK(cudaMemcpyAsync(out->pix_cr, b.pix_cr, ctx->pix_total * 2, cudaMemcpyDeviceToHost, s));
-    if (out->dib)    CK(cudaMemcpyAsync(out->dib,    b.dib,    ctx->dib_total,     cudaMemcpyDeviceToHost, s));
-    if (out->blk_y)  CK(cudaMemcpyAsync(out->blk_y,  b.blk_y,  ctx->blk_total * 2, cudaMemcpyDeviceToHost, s));
-    if (out->blk_cb) CK(cudaMemcpyAsync(out->blk_cb, b.blk_cb, ctx->blk_total * 2, cudaMemcpyDeviceToHost, s));
-    if (out->blk_cr) CK(cudaMemcpyAsync(out->blk_cr, b.blk_cr, ctx->blk_total * 2, cudaMemcpyDeviceToHost, s));
-    if (out->mcu_map) CK(cudaMemcpyAsync(out->mcu_map, b.mcu_map, ctx->mcu_total * 4, cudaMemcpyDeviceToHost, s));
-    if (out->dht_histo) CK(cudaMemcpyAsync(out->dht_histo, b.histo, (size_t)n * 2 * 4 * 17 * 4, cudaMemcpyDeviceToHost, s));
-    if (out->stats)  CK(cudaMemcpyAsync(out->stats, b.stats, (size_t)n * 16 * 4, cudaMemcpyDeviceToHost, s));
-    if (wait) CK(cudaStreamSynchronize(s));
+    for (const JsOutput& o : js_outputs)
+        if (void* h = get_ptr(out, o.host))
+            CK(cudaMemcpyAsync(h, get_ptr(&ctx->batch, o.dev), ctx->plan.*o.total * o.elem, cudaMemcpyDeviceToHost, ctx->stream));
+    if (wait) CK(cudaStreamSynchronize(ctx->stream));
     return JSGPU_OK;
 }
 
-// Host bitstream in, every reference output in host buffers out.  A large batch is cut into JS_HOST_CHUNKS (8) image
-// ranges, each on its own stream with its own pools: the device-to-host copy of one range (PCIe-bound, most of the
-// call) overlaps upload and decode of the next ones.  Afterwards this context holds the batch LAYOUT (and statuses)
-// only; the device pools belong to the chunk contexts, so jsgpu_batch_download()/pools() report JSGPU_ESTATE.
-#define JS_HOST_CHUNKS_MAX 16
+// Host bitstream in, every reference output in host buffers out.  A large batch is cut into JS_HOST_CHUNKS image ranges,
+// each on its own stream with its own pools: the device-to-host copy of one range (PCIe-bound, most of the call) overlaps
+// upload and decode of the next ones.  From the moment it is planned this context holds the batch layout (and, once
+// decoded, the statuses) only: JS_LAYOUT_ONLY.
+#define JS_HOST_CHUNKS 8u
 int jsgpu_decode_batch_host(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32_t n, const uint8_t* bits, uint64_t bytes,
                             const jsgpu_host_outputs* out)
 {
     if (!ctx || !imgs || !bits || !out) return JSGPU_EINVAL;
-    static const uint32_t JS_HOST_CHUNKS = [] { const char* e = getenv("JSGPU_HOST_CHUNKS"); int v = e ? atoi(e) : 8; return (uint32_t)(v < 2 ? 2 : v > JS_HOST_CHUNKS_MAX ? JS_HOST_CHUNKS_MAX : v); }();
     static const uint64_t min_bytes = getenv("JSGPU_HOST_CHUNK_MIN_BYTES") ? strtoull(getenv("JSGPU_HOST_CHUNK_MIN_BYTES"), nullptr, 10) : (64ull << 20);
     bool chunked = n >= 2 * JS_HOST_CHUNKS && bytes >= min_bytes && !ctx->h_sets.empty() && !ctx->h_li.empty();
     for (uint32_t i = 1; chunked && i < n; i++)             // chunk bitstreams must be contiguous, 16-byte aligned ranges
@@ -976,10 +1023,8 @@ int jsgpu_decode_batch_host(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32
     if (!chunked) return decode_host_single(ctx, imgs, n, bits, bytes, out, true);
 
     // global layout (offsets of every image in the host pools) without device allocations
-    ctx->plan_only = true;
-    int r = jsgpu_batch_begin(ctx, imgs, n, bytes);
-    ctx->plan_only = false;
-    if (r) return r;
+    int r = begin_plan(ctx, imgs, n, bytes); if (r) return r;
+    ctx->state = JS_LAYOUT_ONLY;
     while (ctx->kids.size() < JS_HOST_CHUNKS) {
         jsgpu_ctx* k = nullptr;
         r = jsgpu_init(ctx->device, &k); if (r) return fail(ctx, r, "chunk context: %s", jsgpu_strerror(r));
@@ -1001,20 +1046,12 @@ int jsgpu_decode_batch_host(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32
         d.assign(imgs + i0, imgs + i1);
         for (auto& x : d) x.scan_offset -= base;
         uint32_t iv = i0;                                    // first image of the chunk that occupies pool space (skipped images do not)
-        while (iv < i1 && !ctx->himg[iv].valid) iv++;
+        while (iv < i1 && !ctx->plan.img[iv].valid) iv++;
         static const DevImage none = {};
-        const DevImage& f = (iv < i1) ? ctx->himg[iv] : none;    // its offsets in the global pools = where this chunk's outputs start
+        const DevImage& f = (iv < i1) ? ctx->plan.img[iv] : none;    // its offsets in the global pools = where this chunk's outputs start
         jsgpu_host_outputs o2 = {};
-        o2.pix_y  = out->pix_y  ? (int16_t*)out->pix_y  + f.pix_off : nullptr;
-        o2.pix_cb = out->pix_cb ? (int16_t*)out->pix_cb + f.pix_off : nullptr;
-        o2.pix_cr = out->pix_cr ? (int16_t*)out->pix_cr + f.pix_off : nullptr;
-        o2.dib    = out->dib    ? (uint8_t*)out->dib    + f.dib_off : nullptr;
-        o2.blk_y  = out->blk_y  ? (int16_t*)out->blk_y  + f.blk_off : nullptr;
-        o2.blk_cb = out->blk_cb ? (int16_t*)out->blk_cb + f.blk_off : nullptr;
-        o2.blk_cr = out->blk_cr ? (int16_t*)out->blk_cr + f.blk_off : nullptr;
-        o2.mcu_map   = out->mcu_map   ? (uint32_t*)out->mcu_map + f.mcu_off : nullptr;
-        o2.dht_histo = out->dht_histo ? (uint32_t*)out->dht_histo + (size_t)i0 * 2 * 4 * 17 : nullptr;
-        o2.stats     = out->stats     ? (int32_t*)out->stats + (size_t)i0 * 16 : nullptr;
+        for (const JsOutput& o : js_outputs)
+            if (uint8_t* h = (uint8_t*)get_ptr(out, o.host)) set_ptr(&o2, o.host, h + out_off(o, f, i0) * o.elem);
         r = decode_host_single(k, d.data(), i1 - i0, bits + base, end - base, &o2, false);
         if (r) {
             // earlier chunks still have copies in flight into the caller's buffers: let them land before handing control back
@@ -1036,10 +1073,9 @@ int jsgpu_decode_batch_host(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32
         std::vector<jsgpu_image_layout> lo(i1 - i0);
         r = jsgpu_batch_layout(k, lo.data(), i1 - i0);
         if (r) { for (uint32_t c2 = c + 1; c2 < JS_HOST_CHUNKS; c2++) cudaStreamSynchronize(ctx->kids[c2]->stream); return fail(ctx, r, "%s", k->err.c_str()); }
-        for (uint32_t i = i0; i < i1; i++) ctx->layout[i].status = lo[i - i0].status;
+        for (uint32_t i = i0; i < i1; i++) ctx->plan.layout[i].status = lo[i - i0].status;
         ctx->launches += k->launches;
     }
-    ctx->decoded = true; ctx->host_delivered = true;
     return JSGPU_OK;
 }
 

@@ -256,7 +256,7 @@ __global__ void __launch_bounds__(32) k_huff_exact(DevBatch b, int err_max, jsgp
     Ex x;
     x.data = b.bits + im.scan_off; x.n = (uint32_t)im.scan_len; x.file_pos = im.file_pos;
     x.ts = b.tables + im.table_set;
-    x.res = b.ex_res + ii; x.histo = wr ? b.histo + (size_t)ii * 2 * 4 * 17 : scratch_histo;
+    x.res = b.ex_res + ii; x.histo = wr ? b.histo + (size_t)ii * JSGPU_HISTO_WORDS : scratch_histo;
     x.res->nerr_lines = 0; x.res->nevents = 0; x.res->scan_bad = 0; x.res->restart_read = 0; x.res->done = 0;
     x.err_max = (uint32_t)err_max; x.warn_bad_num = 0;
     x.precision = im.precision; x.decode_ac = b.decode_ac != 0;
@@ -315,8 +315,8 @@ __global__ void __launch_bounds__(32) k_huff_exact(DevBatch b, int err_max, jsgp
     if (!wr) return;
     x.res->scan_bad = x.scan_bad ? 1u : 0u; x.res->restart_read = x.restart_read; x.res->done = 1;
     x.res->end_pos = x.pos[0]; x.res->end_align = x.align;
-    b.stats[(size_t)ii * 16 + 11] = (int32_t)x.restart_read;     // m_nRestartRead
-    b.stats[(size_t)ii * 16 + 12] = (int32_t)x.pos[0]; b.stats[(size_t)ii * 16 + 13] = (int32_t)x.align;
+    b.stats[(size_t)ii * JSGPU_STAT_WORDS + 11] = (int32_t)x.restart_read;     // m_nRestartRead
+    b.stats[(size_t)ii * JSGPU_STAT_WORDS + 12] = (int32_t)x.pos[0]; b.stats[(size_t)ii * JSGPU_STAT_WORDS + 13] = (int32_t)x.align;
 }
 
 // Before the re-decode: which images need it, and their intermediates back to the state the reference starts from
@@ -336,7 +336,7 @@ __global__ void __launch_bounds__(256) k_exact_prepare(DevBatch b)
     const size_t nb = (size_t)im.blk_xmax * im.blk_ymax;
     for (size_t i = threadIdx.x; i < nb; i += blockDim.x) { b.blk_y[im.blk_off + i] = 0; if (im.ns == 3) { b.blk_cb[im.blk_off + i] = 0; b.blk_cr[im.blk_off + i] = 0; } }
     for (uint32_t i = threadIdx.x; i < im.nmcu; i += blockDim.x) b.mcu_map[im.mcu_off + i] = 0;
-    for (uint32_t i = threadIdx.x; i < 2 * 4 * 17; i += blockDim.x) b.histo[(size_t)ii * 2 * 4 * 17 + i] = 0;
+    for (uint32_t i = threadIdx.x; i < JSGPU_HISTO_WORDS; i += blockDim.x) b.histo[(size_t)ii * JSGPU_HISTO_WORDS + i] = 0;
 }
 
 int js_launch_exact(const DevBatch& b, int err_max, const jsgpu_detail& dtl, const JsDetailOut& dump, uint32_t* scratch_histo, cudaStream_t s)

@@ -62,7 +62,7 @@ __device__ __forceinline__ void ms_close(const DevBatch& b, uint32_t ii, const D
     for (uint32_t k = nf; k < im.nseg; k++) { seg_start[k] = endpos; seg_end[k] = endpos; }
     b.scan_end[ii] = endpos;
     b.nseg_found[ii] = nf;
-    b.stats[(size_t)ii * 16 + 11] = (int32_t)found;    // m_nRestartRead (ImgDecode.cpp:1414)
+    b.stats[(size_t)ii * JSGPU_STAT_WORDS + 11] = (int32_t)found;    // m_nRestartRead (ImgDecode.cpp:1414)
     if (nf < im.nseg) atomicOr(&b.img_status[ii], 8u);
     if (nf > im.nseg) atomicOr(&b.img_status[ii], 32u);        // more restart markers than intervals: the reference restarts at each one it meets
 }
@@ -382,7 +382,7 @@ __global__ void k_finalize_stats(DevBatch b)
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= b.nimg) return;
     const DevImage& im = b.img[i];
-    int32_t* st = b.stats + (size_t)i * 16;
+    int32_t* st = b.stats + (size_t)i * JSGPU_STAT_WORDS;
     if (!im.valid) return;
     unsigned long long key = b.bright_key[i], sum = b.sum_y[i];
     uint32_t idx = 0xffffffffu - (uint32_t)(key & 0xffffffffu);
@@ -557,8 +557,8 @@ __global__ void __launch_bounds__(256) k_checksums(DevBatch b, unsigned long lon
         case 5: if (c3) s = ck_span(reinterpret_cast<const uint32_t*>(b.blk_cb + im.blk_off), nblk >> 1, nblk & 1, first, step); break;
         case 6: if (c3) s = ck_span(reinterpret_cast<const uint32_t*>(b.blk_cr + im.blk_off), nblk >> 1, nblk & 1, first, step); break;
         case 7: s = ck_span(b.mcu_map + im.mcu_off, im.nmcu, false, first, step); break;
-        case 8: s = ck_span(b.histo + (size_t)ii * 2 * 4 * 17, 2 * 4 * 17, false, first, step); break;
-        case 9: s = ck_span(reinterpret_cast<const uint32_t*>(b.stats + (size_t)ii * 16 + 2), 9, false, first, step); break;    // m_nAvgY, brightest pixel Y/Cb/Cr/R/G/B, its MCU
+        case 8: s = ck_span(b.histo + (size_t)ii * JSGPU_HISTO_WORDS, JSGPU_HISTO_WORDS, false, first, step); break;
+        case 9: s = ck_span(reinterpret_cast<const uint32_t*>(b.stats + (size_t)ii * JSGPU_STAT_WORDS + 2), 9, false, first, step); break;    // m_nAvgY, brightest pixel Y/Cb/Cr/R/G/B, its MCU
         }
         #pragma unroll
         for (int d = 16; d; d >>= 1) s += __shfl_xor_sync(FULL, s, d);
@@ -583,7 +583,7 @@ int js_launch_checksums(const DevBatch& b, unsigned long long* ck, cudaStream_t 
     cudaMemsetAsync(ck, 0, (size_t)b.nimg * JSGPU_CK_WORDS_INTERNAL * 8, s);
     for (uint32_t i0 = 0; i0 < b.nimg; i0 += 65535u) {           // grid.y limit
         DevBatch bb = b; bb.img = b.img + i0; bb.nimg = std::min<uint32_t>(b.nimg - i0, 65535u);
-        bb.histo = b.histo + (size_t)i0 * 2 * 4 * 17; bb.stats = b.stats + (size_t)i0 * 16; bb.img_status = b.img_status + i0;
+        bb.histo = b.histo + (size_t)i0 * JSGPU_HISTO_WORDS; bb.stats = b.stats + (size_t)i0 * JSGPU_STAT_WORDS; bb.img_status = b.img_status + i0;
         k_checksums<<<dim3(32, bb.nimg), 256, 0, s>>>(bb, ck + (size_t)i0 * JSGPU_CK_WORDS_INTERNAL);
     }
     return 1;

@@ -405,47 +405,38 @@ class BatchDecoder:
     def refresh_layout(self):
         self._ck(self.L.jsgpu_batch_layout(self.ctx, C.byref(self.layout), self.n)); return self.layout
 
-    def _dl(self, which, i, dtype, shape):
-        a = np.zeros(shape, dtype)
-        self._ck(self.L.jsgpu_batch_download(self.ctx, which, i, a.ctypes.data, a.nbytes)); return a
+    @staticmethod
+    def _outputs(lo, i):
+        """The ten per-image outputs: (name, JSGPU_OUT_* selector, dtype, shape, element offset of image i in its host pool,
+        absent from a one-component scan).  blk_y/cb/cr become DecodedImage.blk_dc."""
+        W, H = int(lo.img_x), int(lo.img_y); nblk = int(lo.blk_xmax) * int(lo.blk_ymax); nmcu = int(lo.mcu_xmax) * int(lo.mcu_ymax)
+        po, bo = int(lo.pix_off), int(lo.blk_off)
+        return [("pix_y", B.OUT_PIX_Y, np.int16, (H, W), po, False), ("pix_cb", B.OUT_PIX_CB, np.int16, (H, W), po, True),
+                ("pix_cr", B.OUT_PIX_CR, np.int16, (H, W), po, True), ("dib", B.OUT_DIB, np.uint8, (H, W, 4), int(lo.dib_off), False),
+                ("blk_y", B.OUT_BLK_Y, np.int16, (nblk,), bo, False), ("blk_cb", B.OUT_BLK_CB, np.int16, (nblk,), bo, True),
+                ("blk_cr", B.OUT_BLK_CR, np.int16, (nblk,), bo, True),
+                ("mcu_map", B.OUT_MCU_MAP, np.uint32, (nmcu,), int(lo.mcu_off), False),
+                ("dht_histo", B.OUT_HISTO, np.uint32, (2, 4, 17), i * 136, False), ("stats", B.OUT_STATS, np.int32, (16,), i * 16, False)]
+
+    def _image(self, i, get):
+        """DecodedImage of image i, each output from get(name, selector, dtype, shape, offset)."""
+        self.refresh_layout()
+        lo = self.layout[i]; d = DecodedImage()
+        d.geom = np.array([lo.mcu_w, lo.mcu_h, lo.mcu_xmax, lo.mcu_ymax, lo.blk_xmax, lo.blk_ymax, lo.img_x, lo.img_y], np.uint32)
+        ns = self.descs[i].num_sos_comps
+        v = {name: None if chroma and ns != 3 else get(name, sel, dtype, shape, off)
+             for name, sel, dtype, shape, off, chroma in self._outputs(lo, i)}
+        d.blk_dc = (v.pop("blk_y"), v.pop("blk_cb"), v.pop("blk_cr"))
+        d.__dict__.update(v)
+        d.status = int(lo.status)
+        return d
 
     def fetch_host(self, i, outs):
         """The same DecodedImage as fetch(), cut out of the host buffers a decode_host() call filled."""
-        self.refresh_layout()
-        lo = self.layout[i]; d = DecodedImage()
-        d.geom = np.array([lo.mcu_w, lo.mcu_h, lo.mcu_xmax, lo.mcu_ymax, lo.blk_xmax, lo.blk_ymax, lo.img_x, lo.img_y], np.uint32)
-        Wp, Hp = int(lo.img_x), int(lo.img_y); nblk = int(lo.blk_xmax) * int(lo.blk_ymax); nmcu = int(lo.mcu_xmax) * int(lo.mcu_ymax)
-        ns = self.descs[i].num_sos_comps
-        po, do, bo, mo = int(lo.pix_off), int(lo.dib_off), int(lo.blk_off), int(lo.mcu_off)
-        cut = lambda a, off, n, shape: np.array(a[off:off + n]).reshape(shape)
-        d.pix_y = cut(outs["pix_y"], po, Wp * Hp, (Hp, Wp))
-        d.pix_cb = cut(outs["pix_cb"], po, Wp * Hp, (Hp, Wp)) if ns == 3 else None
-        d.pix_cr = cut(outs["pix_cr"], po, Wp * Hp, (Hp, Wp)) if ns == 3 else None
-        d.dib = cut(outs["dib"], do, Wp * Hp * 4, (Hp, Wp, 4))
-        d.mcu_map = cut(outs["mcu_map"], mo, nmcu, (nmcu,))
-        d.blk_dc = (cut(outs["blk_y"], bo, nblk, (nblk,)),
-                    cut(outs["blk_cb"], bo, nblk, (nblk,)) if ns == 3 else None,
-                    cut(outs["blk_cr"], bo, nblk, (nblk,)) if ns == 3 else None)
-        d.dht_histo = cut(outs["dht_histo"], i * 136, 136, (2, 4, 17))
-        d.stats = cut(outs["stats"], i * 16, 16, (16,))
-        d.status = int(lo.status)
-        return d
+        return self._image(i, lambda name, sel, dtype, shape, off: np.array(outs[name][off:off + int(np.prod(shape))]).reshape(shape))
 
     def fetch(self, i):
-        self.refresh_layout()
-        lo = self.layout[i]; d = DecodedImage()
-        d.geom = np.array([lo.mcu_w, lo.mcu_h, lo.mcu_xmax, lo.mcu_ymax, lo.blk_xmax, lo.blk_ymax, lo.img_x, lo.img_y], np.uint32)
-        Wp, Hp = lo.img_x, lo.img_y; nblk = lo.blk_xmax * lo.blk_ymax; nmcu = lo.mcu_xmax * lo.mcu_ymax
-        ns = self.descs[i].num_sos_comps
-        d.pix_y = self._dl(B.OUT_PIX_Y, i, np.int16, (Hp, Wp))
-        d.pix_cb = self._dl(B.OUT_PIX_CB, i, np.int16, (Hp, Wp)) if ns == 3 else None
-        d.pix_cr = self._dl(B.OUT_PIX_CR, i, np.int16, (Hp, Wp)) if ns == 3 else None
-        d.dib = self._dl(B.OUT_DIB, i, np.uint8, (Hp, Wp, 4))
-        d.mcu_map = self._dl(B.OUT_MCU_MAP, i, np.uint32, (nmcu,))
-        d.blk_dc = (self._dl(B.OUT_BLK_Y, i, np.int16, (nblk,)),
-                    self._dl(B.OUT_BLK_CB, i, np.int16, (nblk,)) if ns == 3 else None,
-                    self._dl(B.OUT_BLK_CR, i, np.int16, (nblk,)) if ns == 3 else None)
-        d.dht_histo = self._dl(B.OUT_HISTO, i, np.uint32, (2, 4, 17))
-        d.stats = self._dl(B.OUT_STATS, i, np.int32, (16,))
-        d.status = int(lo.status)
-        return d
+        def dl(name, sel, dtype, shape, off):
+            a = np.zeros(shape, dtype)
+            self._ck(self.L.jsgpu_batch_download(self.ctx, sel, i, a.ctypes.data, a.nbytes)); return a
+        return self._image(i, dl)
