@@ -389,6 +389,23 @@ int jsgpu_decode_batch_host(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32
 int jsgpu_search_bytes(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, const uint8_t* patterns, const uint32_t* lens, uint32_t npat,
                        uint64_t* counts, uint32_t* pos, uint64_t cap);
 
+/* --- value search (Tools -> Img Search Fwd / Rev, JPEGsnoopDoc.cpp:829-932) -----------------------------------------------
+ * Returns what CwindowBuf::BufSearch(start, value, len, forward, found_pos) (WindowBuf.cpp:149-212) returns over the n bytes at
+ * `data` with `noverlays` overlays applied (overlay k replaces overlays[k].len bytes from file offset overlays[k].start, also past
+ * the end of the file; the last one listed wins, as the reference's Buf() does, WindowBuf.cpp:655-681).  Each position p compares the big-endian value of the len (1..4) bytes at p, bytes past
+ * the end of the file reading as 0, with `value`:
+ *   forward  tests start + 1, start + 2, ... and stops after the first p with p + len - 1 >= n (tested too; when
+ *            start + len >= n that is start + 1 alone);
+ *   reverse  tests start - 1 down to 0; from start 0 it tests 0 once.
+ * *found = 1 and *found_pos = the first match in that order, or *found = 0 and *found_pos = the last position tested.
+ * The file is streamed in chunks (JSGPU_SEARCH_CHUNK_BYTES, as jsgpu_search_bytes) in search order through pinned staging
+ * buffers, the overlays patched in on the host; the search stops at the first chunk that holds a match, and no chunk past it
+ * reaches the device.  Files of 2^32 bytes or more and starts of 2^32 - 1 or more are refused (JSGPU_EINVAL): the
+ * reference's positions are 32-bit.  The batch of the context is left untouched.  Synchronous. */
+typedef struct { uint64_t start; uint64_t len; const uint8_t* data; } jsgpu_overlay;
+int jsgpu_find_value(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, uint64_t start, uint32_t value, uint32_t len, int forward,
+                     const jsgpu_overlay* overlays, uint32_t noverlays, int* found, uint64_t* found_pos);
+
 /* Pinned host memory helpers (for callers that want true async copies). */
 void* jsgpu_host_alloc(uint64_t bytes);
 void  jsgpu_host_free(void* p);

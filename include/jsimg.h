@@ -81,6 +81,31 @@ int    jsimg_tiff_write(const char* path, int ycc, int b16, const void* data, un
  * Returns 0, or a negative JSGPU_E* code after one error line and no report (no CUDA device; files of 2^32 bytes or more). */
 int    jsimg_search_dqt(jsimg*, const uint8_t* data, uint64_t n, const char* exe_path, int analysed, const char* analysed_path);
 
+/* Img Search Fwd / Rev and the offset modes (JPEGsnoopDoc.cpp:829-932; JPEGsnoopCore.cpp:700-756).  Positions are absolute
+ * file offsets throughout: a decode at `pos` walks the markers from the SOI at pos, and its scan start, MCU file map, error
+ * lines and Detailed Decode report offsets in the whole file.
+ * jsimg_buf_search: CwindowBuf::BufSearch over the installed file and overlays, on the GPU (jsgpu_find_value); returns 1 found,
+ *   0 not found (*found_pos as the reference leaves it either way) or a negative JSGPU_E* code. */
+int    jsimg_buf_search(jsimg*, uint64_t start, uint32_t value, uint32_t len, int fwd, uint64_t* found_pos);
+/* ProcessFile with nPosStart = pos: the marker walk from the SOI at pos, then DecodeScanImg.  Returns the absolute scan start
+ * or a negative code, as jsimg_decode_jpeg (which is this at pos 0). */
+int    jsimg_decode_jpeg_at(jsimg*, const uint8_t* data, uint64_t n, uint64_t pos, int quiet);
+/* Tools -> Img Search Fwd (fwd = 1) / Rev (fwd = 0) from `start` over the installed file, as the Doc's handlers do it: search
+ * for FF D8 FF; forward, a match becomes the new start and is reprocessed, otherwise nothing changes; reverse (only when
+ * start > 0), a match is reprocessed, otherwise the start becomes 0 and the file is reprocessed from there.  *found: the
+ * search's answer, *pos: the new start, *decoded: whether a decode at *pos ran.  Returns that decode's result (as
+ * jsimg_decode_jpeg), 0 when nothing was decoded, or a negative JSGPU_E* code from the search (with *decoded = 0). */
+int    jsimg_img_search(jsimg*, uint64_t start, int fwd, int quiet, int* found, uint64_t* pos, int* decoded);
+/* DoAnalyzeOffset's modes (teOffsetMode, snoop.h:166): decode at 0; at 0 unless the walk there reaches no frame header
+ * (CjfifDecode::GetDecodeStatus), then at the first FF D8 FF after 0 if there is one; at the first FF D8 FF after 0 if there is
+ * one, else at 0; at `pos`.  *pos_used receives the offset decoded at.  Returns as jsimg_decode_jpeg, or a negative JSGPU_E*
+ * code when a needed search failed (EINVAL for an unknown mode). */
+#define JSIMG_OFFSET_START 0
+#define JSIMG_OFFSET_SRCH1 1
+#define JSIMG_OFFSET_SRCH2 2
+#define JSIMG_OFFSET_POS   3
+int    jsimg_decode_offset_mode(jsimg*, const uint8_t* data, uint64_t n, int mode, uint64_t pos, int quiet, uint64_t* pos_used);
+
 /* log access (error convention: failures are log lines, ImgDecode.cpp:2755-2758 etc.) */
 int    jsimg_log_count(jsimg*, int kind /*0 line,1 hdr,2 warn,3 err,4 good,-1 all*/);
 const char* jsimg_log_line(jsimg*, int kind, int index);
@@ -91,8 +116,10 @@ void   jsimg_log_clear(jsimg*);
  * DecodeScanImg(start, true, quiet) exactly as JfifDecode.cpp:5299 does. */
 int    jsimg_walk_jpeg(jsimg*, const uint8_t* data, uint64_t n);
 int    jsimg_decode_jpeg(jsimg*, const uint8_t* data, uint64_t n, int quiet);
-/* Same walk, but only export the C-ABI table set + image descriptor (for batch decoding). */
+/* Same walk, but only export the C-ABI table set + image descriptor (for batch decoding); _at walks the JPEG whose SOI is at
+ * `pos`, and the scan start it returns and desc->file_pos are absolute file offsets. */
 int    jsimg_parse_jpeg(const uint8_t* data, uint64_t n, jsgpu_tables* tables, jsgpu_image_desc* desc);
+int    jsimg_parse_jpeg_at(const uint8_t* data, uint64_t n, uint64_t pos, jsgpu_tables* tables, jsgpu_image_desc* desc);
 
 #ifdef __cplusplus
 }

@@ -65,6 +65,14 @@ class jsgpu_host_outputs(C.Structure):
                                           "mcu_map", "dht_histo", "stats")]
 
 
+class jsgpu_overlay(C.Structure):
+    _fields_ = [("start", C.c_uint64), ("len", C.c_uint64), ("data", C.c_void_p)]
+
+
+# teOffsetMode (include/jsimg.h JSIMG_OFFSET_*)
+OFFSET_START, OFFSET_SRCH1, OFFSET_SRCH2, OFFSET_POS = range(4)
+
+
 class jsgpu_preview(C.Structure):
     """include/jsgpu.h: CalcChannelPreviewFull settings (histogram/clip conversion, preview mode, YCC shift)."""
     _fields_ = [("hist_en", C.c_int32), ("statclip_en", C.c_int32), ("mode", C.c_int32),
@@ -102,7 +110,7 @@ JSGPU_SYMBOLS = [
     "jsgpu_batch_begin", "jsgpu_batch_layout", "jsgpu_batch_pools", "jsgpu_batch_upload", "jsgpu_batch_decode",
     "jsgpu_batch_download", "jsgpu_batch_stage_ms", "jsgpu_timer_start", "jsgpu_timer_stop", "jsgpu_batch_launches", "jsgpu_batch_selfsync_info", "jsgpu_batch_checksums", "jsgpu_batch_errors", "jsgpu_decode_batch_host",
     "jsgpu_host_alloc", "jsgpu_host_free", "jsgpu_host_copy_rate", "jsgpu_set_preview", "jsgpu_batch_preview", "jsgpu_batch_colour_stats", "jsgpu_batch_export", "jsgpu_set_detail", "jsgpu_batch_detail",
-    "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices", "jsgpu_search_bytes"]
+    "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices", "jsgpu_search_bytes", "jsgpu_find_value"]
 JSIMG_SYMBOLS = [
     "jsimg_create", "jsimg_destroy", "jsimg_config", "jsimg_set_file", "jsimg_overlay_install", "jsimg_overlay_remove_all", "jsimg_Reset", "jsimg_ResetState",
     "jsimg_SetDqtEntry", "jsimg_SetDqtTables", "jsimg_GetDqtEntry", "jsimg_SetDhtTables", "jsimg_SetDhtEntry",
@@ -113,7 +121,7 @@ JSIMG_SYMBOLS = [
     "jsimg_log_count", "jsimg_log_line", "jsimg_log_clear", "jsimg_walk_jpeg", "jsimg_decode_jpeg", "jsimg_parse_jpeg",
     "jsimg_config_histo", "jsimg_SetPreviewMode", "jsimg_GetPreviewMode", "jsimg_SetPreviewYccOffset", "jsimg_GetPreviewYccOffset",
     "jsimg_GetStatClip", "jsimg_GetHistoRanges", "jsimg_GetCcHisto", "jsimg_GetHistoYFull", "jsimg_GetHistoDib", "jsimg_ExportTiff", "jsimg_tiff_write", "jsimg_SetDetailVlc", "jsimg_GetDetailVlc",
-    "jsimg_search_dqt"]
+    "jsimg_search_dqt", "jsimg_buf_search", "jsimg_decode_jpeg_at", "jsimg_img_search", "jsimg_decode_offset_mode", "jsimg_parse_jpeg_at"]
 
 _lib = None
 
@@ -169,6 +177,12 @@ def load():
     L.jsgpu_batch_detail_matrices.argtypes = [vp, u32, u32, vp]
     L.jsgpu_search_bytes.argtypes = [vp, vp, u64, vp, vp, u32, vp, vp, u64]
     L.jsimg_search_dqt.argtypes = [vp, vp, u64, C.c_char_p, i32, C.c_char_p]
+    L.jsgpu_find_value.argtypes = [vp, vp, u64, u64, u32, u32, i32, vp, u32, C.POINTER(i32), C.POINTER(u64)]
+    L.jsimg_buf_search.argtypes = [vp, u64, u32, u32, i32, C.POINTER(u64)]
+    L.jsimg_decode_jpeg_at.argtypes = [vp, vp, u64, u64, i32]
+    L.jsimg_img_search.argtypes = [vp, u64, i32, i32, C.POINTER(i32), C.POINTER(u64), C.POINTER(i32)]
+    L.jsimg_decode_offset_mode.argtypes = [vp, vp, u64, i32, u64, i32, C.POINTER(u64)]
+    L.jsimg_parse_jpeg_at.argtypes = [vp, u64, u64, C.POINTER(jsgpu_tables), C.POINTER(jsgpu_image_desc)]
     L.jsimg_SetDetailVlc.argtypes = [vp, i32, u32, u32, u32]; L.jsimg_SetDetailVlc.restype = None
     L.jsimg_GetDetailVlc.argtypes = [vp] + [C.POINTER(u32)] * 4; L.jsimg_GetDetailVlc.restype = None
     L.jsimg_config_histo.argtypes = [vp, i32, i32, i32]; L.jsimg_config_histo.restype = None

@@ -51,8 +51,11 @@ public:
     }
     bool OverlayInstall(unsigned long start, const uint8_t* d, size_t n) { m_ovl.push_back({start, std::vector<uint8_t>(d, d + n)}); return true; }
     void OverlayRemoveAll() { m_ovl.clear(); }
-private:
+    // the file and the overlays in installed order, for searches that stream the whole file (jsimg_buf_search)
     struct Ovl { unsigned long start; std::vector<uint8_t> data; };
+    const uint8_t* BufData() const { return m_p; }
+    const std::vector<Ovl>& Overlays() const { return m_ovl; }
+private:
     const uint8_t* m_p = nullptr; size_t m_n = 0;
     std::vector<Ovl> m_ovl;
 };

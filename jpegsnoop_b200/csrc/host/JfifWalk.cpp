@@ -10,13 +10,17 @@ const unsigned kJfifZigZag[64] = {
      0, 1, 8,16, 9, 2, 3,10, 17,24,32,25,18,11, 4, 5, 12,19,26,33,40,48,41,34, 27,20,13, 6, 7,14,21,28,
     35,42,49,56,57,50,43,36, 29,22,15,23,30,37,44,51, 58,59,52,45,38,31,39,46, 53,60,61,54,47,55,62,63 };
 
-int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n)
+int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n, uint64_t nPosStart, bool* pbSof)
 {
     unsigned unzz[64];
     for (unsigned i = 0; i < 64; i++) unzz[kJfifZigZag[i]] = i;
     pImgDec->ResetState();
-    if (n < 4 || d[0] != 0xFF || d[1] != 0xD8) return JFIFWALK_ENOTJPEG;
-    uint64_t p = 2;
+    bool bSofSeen = false;                                          // CjfifDecode::m_bImgOK (JfifDecode.cpp:96, 5030)
+    if (!pbSof) pbSof = &bSofSeen;
+    *pbSof = false;
+    // ProcessFile starts the marker walk at m_pAppConfig->nPosStart and every position stays absolute (JfifDecode.cpp:7338-7341)
+    if (nPosStart >= n || n - nPosStart < 4 || d[nPosStart] != 0xFF || d[nPosStart + 1] != 0xD8) return JFIFWALK_ENOTJPEG;
+    uint64_t p = nPosStart + 2;
     unsigned X = 0, Y = 0, Nf = 0, P = 8, nRstInterval = 0;
     bool bRstEn = false, bSof = false;
     while (p + 4 <= n) {
@@ -49,9 +53,10 @@ int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n)
             for (unsigned i = 1; i <= Nf; i++) { q++; H[i] = d[q] >> 4; V[i] = d[q] & 15; q++; T[i] = d[q++]; }
             for (unsigned i = 1; i <= Nf; i++) { pImgDec->SetDqtTables(i, T[i]); pImgDec->SetPrecision(P); }       // :5008,5012
             for (unsigned i = 1; i <= Nf; i++) pImgDec->SetSofSampFactors(i, H[i], V[i]);                           // :5025
-            bSof = true;
+            bSof = true; *pbSof = true;
             break; }
         case 0xC2: case 0xC3: case 0xC5: case 0xC6: case 0xC7: case 0xC9: case 0xCA: case 0xCB: case 0xCD: case 0xCE: case 0xCF:
+            *pbSof = true;                                          // the reference parses these frames too (:4800-4812)
             return JFIFWALK_EUNSUP;
         case 0xC4:                                                  // DHT
             while (q < e) {

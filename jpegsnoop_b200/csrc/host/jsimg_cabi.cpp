@@ -8,7 +8,7 @@
 
 struct jsimg {
     CDocLog log; CwindowBuf wbuf; CSnoopConfig cfg; CimgDecode* dec;
-    jsgpu_ctx* search = nullptr;        // the byte-pattern search's device context (jsimg_search_dqt), created on first use
+    jsgpu_ctx* search = nullptr;        // the searches' device context (jsimg_search_dqt, jsimg_buf_search), created on first use
     jsimg() : dec(new CimgDecode(&log, &wbuf, &cfg)) {}
     ~jsimg() { delete dec; if (search) jsgpu_free(search); }
 };
@@ -83,22 +83,86 @@ const char* jsimg_log_line(jsimg* h, int kind, int index)
 void jsimg_log_clear(jsimg* h) { h->log.Clear(); }
 
 int jsimg_walk_jpeg(jsimg* h, const uint8_t* d, uint64_t n) { jsimg_set_file(h, d, n); return JfifWalk(h->dec, d, n); }
-int jsimg_decode_jpeg(jsimg* h, const uint8_t* d, uint64_t n, int quiet)
+// ProcessFile with nPosStart = pos over the installed file: the walk, then DecodeScanImg at the scan's absolute offset
+static int decode_at(jsimg* h, uint64_t pos, int quiet)
 {
-    int start = jsimg_walk_jpeg(h, d, n);
+    const int start = JfifWalk(h->dec, h->wbuf.BufData(), h->wbuf.GetPosEof(), pos);
     if (start < 0) return start;
     h->dec->DecodeScanImg((unsigned)start, true, quiet != 0);       // JfifDecode.cpp:5299
     return start;
+}
+int jsimg_decode_jpeg(jsimg* h, const uint8_t* d, uint64_t n, int quiet) { return jsimg_decode_jpeg_at(h, d, n, 0, quiet); }
+int jsimg_decode_jpeg_at(jsimg* h, const uint8_t* d, uint64_t n, uint64_t pos, int quiet) { jsimg_set_file(h, d, n); return decode_at(h, pos, quiet); }
+int jsimg_buf_search(jsimg* h, uint64_t start, uint32_t value, uint32_t len, int fwd, uint64_t* found_pos)
+{
+    if (!h->search) {
+        const int r = jsgpu_init(h->cfg.nCudaDevice, &h->search);
+        if (r != JSGPU_OK) {
+            h->search = nullptr;
+            h->log.AddLineErr(std::string("*** ERROR: Img Search: GPU search unavailable (") + jsgpu_strerror(r) + ") ***");
+            return r;
+        }
+    }
+    std::vector<jsgpu_overlay> ovl;
+    for (auto& o : h->wbuf.Overlays()) ovl.push_back({(uint64_t)o.start, (uint64_t)o.data.size(), o.data.data()});
+    int found = 0;
+    const int r = jsgpu_find_value(h->search, h->wbuf.BufData(), h->wbuf.GetPosEof(), start, value, len, fwd, ovl.data(),
+                                   (uint32_t)ovl.size(), &found, found_pos);
+    if (r != JSGPU_OK) {
+        h->log.AddLineErr(std::string("*** ERROR: Img Search: ") + jsgpu_strerror(r) + " (" + jsgpu_last_error(h->search) + ") ***");
+        return r;
+    }
+    return found;
+}
+int jsimg_img_search(jsimg* h, uint64_t start, int fwd, int quiet, int* found, uint64_t* pos, int* decoded)
+{
+    *found = 0; *pos = start; *decoded = 0;
+    if (!fwd && start == 0) return 0;                               // "Don't attempt to search past start of file" (JPEGsnoopDoc.cpp:902)
+    uint64_t p = 0;
+    const int r = jsimg_buf_search(h, start, 0xFFD8FF, 3, fwd, &p);
+    if (r < 0) return r;
+    *found = r;
+    if (r) *pos = p;
+    else if (fwd) return 0;                                         // forward: the start stays, nothing is reprocessed
+    else *pos = 0;                                                  // reverse: reprocess from the start of the file
+    *decoded = 1;
+    return decode_at(h, *pos, quiet);
+}
+int jsimg_decode_offset_mode(jsimg* h, const uint8_t* d, uint64_t n, int mode, uint64_t pos, int quiet, uint64_t* pos_used)
+{
+    jsimg_set_file(h, d, n);
+    *pos_used = 0;
+    uint64_t at = 0, p = 0;
+    int r = 0;
+    switch (mode) {                                                 // CJPEGsnoopCore::DoAnalyzeOffset (JPEGsnoopCore.cpp:700-756)
+    case JSIMG_OFFSET_START: break;
+    case JSIMG_OFFSET_SRCH1: {                                      // search only when the decode at 0 did not reach a frame header
+        bool bImgOK = false;
+        JfifWalk(h->dec, d, n, 0, &bImgOK);
+        if (bImgOK) break;
+        if ((r = jsimg_buf_search(h, 0, 0xFFD8FF, 3, 1, &p)) < 0) return r;
+        if (r) at = p;
+        break; }
+    case JSIMG_OFFSET_SRCH2:                                        // the first SOI after offset 0
+        if ((r = jsimg_buf_search(h, 0, 0xFFD8FF, 3, 1, &p)) < 0) return r;
+        if (r) at = p;
+        break;
+    case JSIMG_OFFSET_POS: at = pos; break;
+    default: return JSGPU_EINVAL;
+    }
+    *pos_used = at;
+    return decode_at(h, at, quiet);
 }
 int jsimg_search_dqt(jsimg* h, const uint8_t* d, uint64_t n, const char* exe_path, int analysed, const char* analysed_path)
 {
     return DqtSearch(&h->log, &h->search, h->cfg.nCudaDevice, analysed ? h->dec : nullptr, d, n, exe_path, analysed_path);
 }
-int jsimg_parse_jpeg(const uint8_t* d, uint64_t n, jsgpu_tables* t, jsgpu_image_desc* desc)
+int jsimg_parse_jpeg(const uint8_t* d, uint64_t n, jsgpu_tables* t, jsgpu_image_desc* desc) { return jsimg_parse_jpeg_at(d, n, 0, t, desc); }
+int jsimg_parse_jpeg_at(const uint8_t* d, uint64_t n, uint64_t pos, jsgpu_tables* t, jsgpu_image_desc* desc)
 {
     CDocLog log; CwindowBuf wb; CSnoopConfig cfg; wb.BufSet(d, (size_t)n);
     CimgDecode dec(&log, &wb, &cfg);
-    int start = JfifWalk(&dec, d, n);
+    int start = JfifWalk(&dec, d, n, pos);
     if (start < 0) return start;
     dec.ExportTables(*t);
     if (!dec.ExportImageDesc(*desc, (unsigned)start)) return JFIFWALK_EMARKER;

@@ -1119,6 +1119,21 @@ int jsgpu_search_bytes(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, const ui
     return js_search_run(&ctx->search, ctx->device, ctx->sm_count, data, n, patterns, lens, npat, counts, pos, cap, ctx->err);
 }
 
+int jsgpu_find_value(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, uint64_t start, uint32_t value, uint32_t len, int forward,
+                     const jsgpu_overlay* overlays, uint32_t noverlays, int* found, uint64_t* found_pos)
+{
+    if (!ctx) return JSGPU_EINVAL;
+    if (!found || !found_pos || (n && !data) || (noverlays && !overlays) || len < 1 || len > 4)
+        return fail(ctx, JSGPU_EINVAL, "jsgpu_find_value: bad arguments (len %u, 1..4)", len);
+    for (uint32_t k = 0; k < noverlays; k++)
+        if (overlays[k].len && !overlays[k].data) return fail(ctx, JSGPU_EINVAL, "jsgpu_find_value: overlay %u has no data", k);
+    if ((n >> 32) || start >= 0xFFFFFFFFull)
+        return fail(ctx, JSGPU_EINVAL, "jsgpu_find_value: %llu bytes from %llu: files of 2^32 bytes or more do not fit 32-bit offsets",
+                    (unsigned long long)n, (unsigned long long)start);
+    return js_find_run(&ctx->search, ctx->device, ctx->sm_count, data, n, start, value, len, forward, overlays, noverlays, found,
+                       found_pos, ctx->err);
+}
+
 void* jsgpu_host_alloc(uint64_t bytes) { void* p = nullptr; if (cudaMallocHost(&p, bytes) != cudaSuccess) return nullptr; return p; }
 void  jsgpu_host_free(void* p) { if (p) cudaFreeHost(p); }
 

@@ -18,6 +18,7 @@
 //                          anything, in file order, into a compact per-chunk list the host copies into place.
 // Device memory is two chunk buffers, the per-tile summaries and one chunk's emitted positions, whatever the file size.
 // The search has its own streams and buffers: a batch resident on the same context is not touched.
+// The first-match value search of Img Search Fwd / Rev (jsgpu_find_value, end of file) shares them.
 #include "jsgpu_internal.h"
 #include <cstdlib>
 #include <cstring>
@@ -269,6 +270,7 @@ struct JsSearch {
     uint8_t* dpat = nullptr; uint32_t* dhash = nullptr;
     uint32_t* dres = nullptr; size_t res_cap = 0;
     uint32_t* dout = nullptr; size_t out_cap = 0;
+    uint32_t* dfind = nullptr; uint32_t* hfind = nullptr;   // jsgpu_find_value: one result word per slot, device and pinned host
 };
 
 void js_search_free(JsSearch* s)
@@ -282,7 +284,7 @@ void js_search_free(JsSearch* s)
         if (s->scanned[i]) cudaEventDestroy(s->scanned[i]);
         if (s->st[i]) cudaStreamDestroy(s->st[i]);
     }
-    cudaFree(s->dpat); cudaFree(s->dhash); cudaFree(s->dres); cudaFree(s->dout);
+    cudaFree(s->dpat); cudaFree(s->dhash); cudaFree(s->dres); cudaFree(s->dout); cudaFree(s->dfind); cudaFreeHost(s->hfind);
     delete s;
 }
 
@@ -306,24 +308,52 @@ template <typename T> static cudaError_t sr_grow(T*& p, size_t& cap, size_t n)
     return e;
 }
 
+#define SR_TRY(call) do { const int r_ = (call); if (r_ != JSGPU_OK) return r_; } while (0)
+
+// the search's streams, events and small buffers, created on the context's first search
+static int sr_open(JsSearch** ps, int device, std::string& err)
+{
+    cudaSetDevice(device);
+    if (*ps) return JSGPU_OK;
+    JsSearch* s = new JsSearch(); s->device = device;
+    *ps = s;
+    for (int i = 0; i < 2; i++) {
+        SR_CK(cudaStreamCreateWithFlags(&s->st[i], cudaStreamNonBlocking));
+        SR_CK(cudaEventCreateWithFlags(&s->copied[i], cudaEventDisableTiming));
+        SR_CK(cudaEventCreateWithFlags(&s->scanned[i], cudaEventDisableTiming));
+    }
+    size_t c0 = 0, c1 = 0, c2 = 0;
+    SR_CK(sr_grow(s->dpat, c0, (size_t)JSGPU_SEARCH_MAX_PATTERNS * 256));
+    SR_CK(sr_grow(s->dhash, c1, (size_t)(1u << SR_HBITS) / 32));
+    SR_CK(sr_grow(s->dfind, c2, 2));
+    SR_CK(cudaMallocHost((void**)&s->hfind, 2 * sizeof(uint32_t)));
+    return JSGPU_OK;
+}
+
+// two pinned staging buffers of at least `pin` bytes and two device chunk buffers of at least `dev` bytes
+static int sr_reserve(JsSearch* s, size_t pin, size_t dev, std::string& err)
+{
+    if (s->pin_cap < pin) {
+        for (int i = 0; i < 2; i++) { cudaFreeHost(s->pin[i]); s->pin[i] = nullptr; }
+        s->pin_cap = 0;
+        for (int i = 0; i < 2; i++) SR_CK(cudaMallocHost((void**)&s->pin[i], pin));
+        s->pin_cap = pin;
+    }
+    if (s->dbuf_cap < dev) {
+        for (int i = 0; i < 2; i++) { cudaFree(s->dbuf[i]); s->dbuf[i] = nullptr; }
+        s->dbuf_cap = 0;
+        for (int i = 0; i < 2; i++) SR_CK(cudaMalloc((void**)&s->dbuf[i], dev));
+        s->dbuf_cap = dev;
+    }
+    return JSGPU_OK;
+}
+
 int js_search_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, uint64_t n, const uint8_t* pats, const uint32_t* lens,
                   uint32_t npat, uint64_t* counts, uint32_t* pos, uint64_t cap, std::string& err)
 {
     for (uint32_t k = 0; k < npat; k++) counts[k] = 0;
     if (n == 0) return JSGPU_OK;
-    cudaSetDevice(device);
-    if (!*ps) {
-        JsSearch* s = new JsSearch(); s->device = device;
-        *ps = s;
-        for (int i = 0; i < 2; i++) {
-            SR_CK(cudaStreamCreateWithFlags(&s->st[i], cudaStreamNonBlocking));
-            SR_CK(cudaEventCreateWithFlags(&s->copied[i], cudaEventDisableTiming));
-            SR_CK(cudaEventCreateWithFlags(&s->scanned[i], cudaEventDisableTiming));
-        }
-        size_t c0 = 0, c1 = 0;
-        SR_CK(sr_grow(s->dpat, c0, (size_t)JSGPU_SEARCH_MAX_PATTERNS * 256));
-        SR_CK(sr_grow(s->dhash, c1, (size_t)(1u << SR_HBITS) / 32));
-    }
+    SR_TRY(sr_open(ps, device, err));
     JsSearch* s = *ps;
 
     // patterns, their prefix hash and the reporting limits
@@ -347,18 +377,7 @@ int js_search_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, 
     const uint32_t nchunks = (uint32_t)((n + chunk - 1) / chunk);
     const uint32_t tiles = (uint32_t)(chunk / SR_TILE);
     const size_t span = chunk + P.maxlen - 1;                 // bytes uploaded per chunk
-    if (s->pin_cap < span) {
-        for (int i = 0; i < 2; i++) { cudaFreeHost(s->pin[i]); s->pin[i] = nullptr; }
-        s->pin_cap = 0;
-        for (int i = 0; i < 2; i++) SR_CK(cudaMallocHost((void**)&s->pin[i], span));
-        s->pin_cap = span;
-    }
-    if (s->dbuf_cap < span) {
-        for (int i = 0; i < 2; i++) { cudaFree(s->dbuf[i]); s->dbuf[i] = nullptr; }
-        s->dbuf_cap = 0;
-        for (int i = 0; i < 2; i++) SR_CK(cudaMalloc((void**)&s->dbuf[i], span));
-        s->dbuf_cap = span;
-    }
+    SR_TRY(sr_reserve(s, span, span, err));
     const size_t tneed = (size_t)tiles * npat;
     if (s->tile_cap < tneed) {
         for (int i = 0; i < 2; i++) { cudaFree(s->dsum[i]); cudaFree(s->doff[i]); s->dsum[i] = s->doff[i] = nullptr; }
@@ -435,5 +454,149 @@ int js_search_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, 
         }
     }
     SR_CK(cudaStreamSynchronize(s->st[0])); SR_CK(cudaStreamSynchronize(s->st[1]));
+    return JSGPU_OK;
+}
+
+// ---- value search (jsgpu_find_value, include/jsgpu.h) -----------------------------------------------------------------
+// CwindowBuf::BufSearch (WindowBuf.cpp:149-212) compares the big-endian value of the `len` bytes at each position with the
+// value, one position at a time, forward from start + 1 or backward from start - 1, and stops at the first match.  Here the
+// positions whose bytes all lie inside the file are searched on the device, chunk by chunk in search order; the few that
+// read past the end of the file (as 0, WindowBuf.cpp:704-711) are tested on the host.
+#define FV_THREADS 256
+#define FV_TILE    (FV_THREADS * 16)     // 16 consecutive positions per thread
+
+// Positions 0 .. npos-1 of one chunk: buf holds their npos + len - 1 bytes and is readable up to 20 bytes past the last
+// 16-byte group.  A position matches when its four bytes, little-endian and masked to len bytes, equal `pat`.
+// res receives the lowest match (forward) or the highest match + 1 (reverse) if it beats what is there.
+__global__ void __launch_bounds__(FV_THREADS)
+k_find_value(const uint8_t* __restrict__ buf, uint32_t npos, uint32_t pat, uint32_t mask, int forward, uint32_t* __restrict__ res)
+{
+    __shared__ uint32_t s_best;                              // forward: lowest match, ~0 for none; reverse: highest + 1, 0 for none
+    const uint32_t tid = threadIdx.x, lane = tid & 31, none = forward ? 0xFFFFFFFFu : 0u;
+    if (tid == 0) s_best = none;
+    __syncthreads();
+    const uint32_t ntiles = (npos + FV_TILE - 1) / FV_TILE;
+    // tiles in search order, so that a CTA can stop at its first tile with a match
+    for (uint32_t i = blockIdx.x; i < ntiles; i += gridDim.x) {
+        const uint32_t t = forward ? i : ntiles - 1 - i;
+        const uint32_t p0 = t * FV_TILE + 16 * tid;
+        uint32_t m = 0;
+        if (p0 < npos) {
+            const uint4 a = *(const uint4*)(buf + p0);
+            const uint32_t w[5] = {a.x, a.y, a.z, a.w, *(const uint32_t*)(buf + p0 + 16)};
+#pragma unroll
+            for (int k = 0; k < 16; k++) {
+                const uint32_t v = (k % 4) ? __funnelshift_r(w[k / 4], w[k / 4 + 1], 8 * (k % 4)) : w[k / 4];
+                if ((v & mask) == pat) m |= 1u << k;
+            }
+            if (npos - p0 < 16) m &= (1u << (npos - p0)) - 1u;
+        }
+        const uint32_t vote = __ballot_sync(0xffffffffu, m != 0);
+        if (vote && lane == (uint32_t)(forward ? __ffs(vote) - 1 : 31 - __clz(vote))) {
+            if (forward) atomicMin(&s_best, p0 + __ffs(m) - 1);
+            else         atomicMax(&s_best, p0 + (31 - __clz(m)) + 1);
+        }
+        if (__syncthreads_or(m != 0)) break;                 // every later tile of this CTA lies further in search order
+    }
+    __syncthreads();
+    if (tid == 0 && s_best != none) {
+        if (forward) atomicMin(res, s_best);
+        else         atomicMax(res, s_best);
+    }
+}
+
+int js_find_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, uint64_t n, uint64_t start, uint32_t value,
+                uint32_t len, int forward, const jsgpu_overlay* ovl, uint32_t novl, int* found, uint64_t* found_pos, std::string& err)
+{
+    // Buf(): the file byte, 0 past EOF, replaced by the last enabled overlay that covers it (WindowBuf.cpp:655-681)
+    auto byte_at = [&](uint64_t q) {
+        uint8_t b = q < n ? data[q] : 0;
+        for (uint32_t k = 0; k < novl; k++) if (q >= ovl[k].start && q - ovl[k].start < ovl[k].len) b = ovl[k].data[q - ovl[k].start];
+        return b;
+    };
+    auto test = [&](uint64_t p) { uint32_t v = 0; for (uint32_t i = 0; i < len; i++) v = (v << 8) | byte_at(p + i); return v == value; };
+    const uint32_t mask = len == 4 ? 0xFFFFFFFFu : (1u << (8 * len)) - 1u;
+    const bool possible = (value & ~mask) == 0;               // a value wider than len bytes never matches
+    const int64_t inside = (int64_t)n - (int64_t)len;         // the last position whose bytes all lie in the file
+    *found = 0;
+
+    // the positions the device searches, [lo, hi], and what the host tests around them
+    int64_t lo = 0, hi = -1;
+    if (forward) {
+        // start + 1, start + 2, ... up to and including the first position that reads past EOF (or start + 1 alone)
+        const int64_t first = (int64_t)start + 1, last = std::max(first, inside + 1);
+        *found_pos = (uint64_t)last;
+        if (!possible) return JSGPU_OK;
+        lo = first; hi = last - 1;
+    } else {
+        *found_pos = 0;                                       // the reference stops at 0 (from 0 it tests 0 once)
+        if (!possible) return JSGPU_OK;
+        int64_t p = start ? (int64_t)start - 1 : 0;
+        // positions that read past EOF, from the top: past the file and every overlay the bytes are all 0
+        while (p > inside && p >= 0) {
+            bool touched = p < (int64_t)n;
+            int64_t next = (int64_t)n - 1;                    // the next lower position whose bytes can differ from 0
+            for (uint32_t k = 0; k < novl; k++) {
+                const int64_t s0 = (int64_t)ovl[k].start - (int64_t)len + 1, s1 = (int64_t)(ovl[k].start + ovl[k].len) - 1;
+                if (p >= s0 && p <= s1) touched = true;
+                if (s0 <= p - 1) next = std::max(next, std::min(s1, p - 1));
+            }
+            if (touched ? test((uint64_t)p) : value == 0) { *found = 1; *found_pos = (uint64_t)p; return JSGPU_OK; }
+            if (!start) return JSGPU_OK;
+            p = touched ? p - 1 : next;
+        }
+        if (!start) { *found = test(0); return JSGPU_OK; }
+        lo = 0; hi = p;
+    }
+
+    if (hi >= lo) {
+        SR_TRY(sr_open(ps, device, err));
+        JsSearch* s = *ps;
+        const uint64_t range = (uint64_t)(hi - lo + 1);
+        const uint64_t chunk = std::min<uint64_t>(sr_chunk_bytes(), (range + FV_TILE - 1) / FV_TILE * FV_TILE);
+        const uint64_t nchunks = (range + chunk - 1) / chunk;
+        SR_TRY(sr_reserve(s, chunk + 3, chunk + 64, err));
+        int occ = 0;
+        SR_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_find_value, FV_THREADS, 0));
+        const uint32_t grid_max = (uint32_t)(std::max(occ, 1) * sm_count);
+        const uint32_t pat = __builtin_bswap32(value) >> (32 - 8 * len);      // the bytes in file order, little-endian
+        // chunk c in search order: positions [plo, phi], bytes [plo, phi + len - 1] (its len - 1 halo bytes lie in the file)
+        auto bounds = [&](uint64_t c, uint64_t& plo, uint64_t& phi) {
+            if (forward) { plo = (uint64_t)lo + c * chunk; phi = std::min<uint64_t>((uint64_t)hi, plo + chunk - 1); }
+            else         { phi = (uint64_t)hi - c * chunk; plo = phi + 1 > (uint64_t)lo + chunk ? phi + 1 - chunk : (uint64_t)lo; }
+        };
+        auto stage = [&](uint64_t c) {
+            uint64_t plo, phi; bounds(c, plo, phi);
+            const uint64_t nb = phi - plo + len;
+            uint8_t* dst = s->pin[c & 1];
+            memcpy(dst, data + plo, nb);
+            for (uint32_t k = 0; k < novl; k++) {                  // installed order: the last overlay wins
+                const uint64_t a = std::max<uint64_t>(ovl[k].start, plo), b = std::min<uint64_t>(ovl[k].start + ovl[k].len, plo + nb);
+                if (a < b) memcpy(dst + (a - plo), ovl[k].data + (a - ovl[k].start), b - a);
+            }
+        };
+        // The host stages chunk c + 1 while the device searches chunk c; chunk c + 1 goes to the device only if c has no match.
+        stage(0);
+        for (uint64_t c = 0; c < nchunks; c++) {
+            const int sl = (int)(c & 1);
+            uint64_t plo, phi; bounds(c, plo, phi);
+            const uint32_t npos = (uint32_t)(phi - plo + 1);
+            SR_CK(cudaMemcpyAsync(s->dbuf[sl], s->pin[sl], npos + len - 1, cudaMemcpyHostToDevice, s->st[sl]));
+            SR_CK(cudaMemsetAsync(s->dfind + sl, forward ? 0xFF : 0, 4, s->st[sl]));
+            const uint32_t grid = std::max(1u, std::min(grid_max, (npos + FV_TILE - 1) / FV_TILE));
+            k_find_value<<<grid, FV_THREADS, 0, s->st[sl]>>>(s->dbuf[sl], npos, pat, mask, forward, s->dfind + sl);
+            SR_CK(cudaGetLastError());
+            SR_CK(cudaMemcpyAsync(s->hfind + sl, s->dfind + sl, 4, cudaMemcpyDeviceToHost, s->st[sl]));
+            SR_CK(cudaEventRecord(s->copied[sl], s->st[sl]));
+            if (c + 1 < nchunks) stage(c + 1);                    // the other slot's chunk finished in the previous round
+            SR_CK(cudaEventSynchronize(s->copied[sl]));
+            const uint32_t r = s->hfind[sl];
+            if (forward ? r != 0xFFFFFFFFu : r != 0u) {
+                *found = 1; *found_pos = plo + (forward ? r : r - 1);
+                return JSGPU_OK;
+            }
+        }
+    }
+    if (forward) *found = test(*found_pos);                  // the last position, which reads past EOF
     return JSGPU_OK;
 }

@@ -20,7 +20,7 @@ class DecodedImage:
     def __init__(self):
         self.geom = None; self.pix_y = self.pix_cb = self.pix_cr = None; self.dib = None
         self.mcu_map = None; self.blk_dc = None; self.dht_histo = None; self.stats = None
-        self.nerr = 0; self.scan_start = 0; self.status = 0; self.stage_ms = None
+        self.nerr = 0; self.scan_start = 0; self.status = 0; self.stage_ms = None; self.pos = 0
 
 
 class CimgDecode:
@@ -31,6 +31,7 @@ class CimgDecode:
         self.h = C.c_void_p(self.L.jsimg_create())
         self.L.jsimg_config(self.h, int(decode_ac), int(idct_fixedpt), device, huff_kernel, idct_kernel, 1)
         self._file = None
+        self.reprocessed = None
 
     def close(self):
         if self.h:
@@ -182,25 +183,64 @@ class CimgDecode:
         d.nerr = self.num_err_lines(); d.status = int(self.L.jsimg_GetScanStatus(self.h))
         return d
 
-    def decode(self, jpeg_bytes, quiet=True):
-        """Marker walk (CjfifDecode's setter sequence) then DecodeScanImg(start, True, quiet)."""
+    def decode(self, jpeg_bytes, quiet=True, offset=0, mode=None):
+        """Marker walk (CjfifDecode's setter sequence) from the SOI at `offset`, then DecodeScanImg(start, True, quiet).
+        With `mode` (B.OFFSET_START / SRCH1 / SRCH2 / POS, DoAnalyzeOffset's modes) the offset is chosen as the reference's
+        command line does; `offset` is then the position of OFFSET_POS.  Every position is absolute in `jpeg_bytes`;
+        d.pos is the offset decoded at."""
         self.set_file(jpeg_bytes)
         self.L.jsimg_log_clear(self.h)
-        r = self.L.jsimg_decode_jpeg(self.h, self._file.ctypes.data, self._file.size, int(quiet))
+        if mode is None:
+            r = self.L.jsimg_decode_jpeg_at(self.h, self._file.ctypes.data, self._file.size, offset, int(quiet))
+            pos = offset
+        else:
+            used = C.c_uint64(0)
+            r = self.L.jsimg_decode_offset_mode(self.h, self._file.ctypes.data, self._file.size, mode, offset, int(quiet), C.byref(used))
+            pos = used.value
         if r < 0:
-            raise ValueError(f"marker walk failed ({r})")
-        d = self.collect(); d.scan_start = r
+            raise ValueError(f"marker walk failed ({r}) at offset {pos}: {self.log_lines(3)}")
+        d = self.collect(); d.scan_start = r; d.pos = pos
         return d
 
+    def buf_search(self, start, value, length, forward=True):
+        """CwindowBuf::BufSearch over the file set last and its overlays, on the GPU: (found, position)."""
+        p = C.c_uint64(0)
+        r = self.L.jsimg_buf_search(self.h, start, value, length, int(forward), C.byref(p))
+        if r < 0:
+            raise JsgpuError(f"jsimg_buf_search failed ({r}): {self.log_lines(3)}")
+        return bool(r), p.value
 
-def parse_jpeg(jpeg_bytes):
-    """Marker walk only -> (jsgpu_tables, jsgpu_image_desc, scan_start)."""
+    def _img_search(self, start, forward, quiet):
+        found, pos, decoded = C.c_int(0), C.c_uint64(0), C.c_int(0)
+        self.L.jsimg_log_clear(self.h)
+        r = self.L.jsimg_img_search(self.h, start, int(forward), int(quiet), C.byref(found), C.byref(pos), C.byref(decoded))
+        if r < 0 and not decoded.value:
+            raise JsgpuError(f"jsimg_img_search failed ({r}): {self.log_lines(3)}")
+        # the scan start of the reprocessed image (negative: its marker walk failed), or None when nothing was reprocessed
+        self.reprocessed = r if decoded.value else None
+        return bool(found.value), pos.value
+
+    def search_forward(self, start, quiet=False):
+        """Tools -> Img Search Fwd from `start` over the file set last (JPEGsnoopDoc.cpp:828-873): (found, new start).  A match
+        is reprocessed (self.reprocessed is its scan start; collect() returns its outputs); otherwise nothing changes.  The
+        reprocess writes the scan-decode lines the reference's Reprocess writes (DecodeScanImg with bQuiet false)."""
+        return self._img_search(start, True, quiet)
+
+    def search_reverse(self, start, quiet=False):
+        """Tools -> Img Search Rev (JPEGsnoopDoc.cpp:878-932): (found, new start).  From start > 0 a match is reprocessed, and
+        without one the file is reprocessed from 0; from start 0 nothing happens (self.reprocessed is None)."""
+        return self._img_search(start, False, quiet)
+
+
+def parse_jpeg(jpeg_bytes, offset=0):
+    """Marker walk only, from the SOI at `offset` -> (jsgpu_tables, jsgpu_image_desc, scan_start); the scan start and
+    desc.file_pos are absolute offsets in `jpeg_bytes`."""
     L = B.load()
     buf = np.frombuffer(bytes(jpeg_bytes), np.uint8)
     t = B.jsgpu_tables(); d = B.jsgpu_image_desc()
-    r = L.jsimg_parse_jpeg(buf.ctypes.data, buf.size, C.byref(t), C.byref(d))
+    r = L.jsimg_parse_jpeg_at(buf.ctypes.data, buf.size, offset, C.byref(t), C.byref(d))
     if r < 0:
-        raise ValueError(f"marker walk failed ({r})")
+        raise ValueError(f"marker walk failed ({r}) at offset {offset}")
     return t, d, r
 
 
@@ -260,10 +300,13 @@ class BatchDecoder:
     @staticmethod
     def prepare(jpegs):
         """Host-side preparation: marker walk of every JPEG, table-set dedupe, concatenation of the
-        scan bytes.  Returns (table_sets array, descs array, bitstream uint8 array)."""
+        scan bytes.  Returns (table_sets array, descs array, bitstream uint8 array).  An entry may be a
+        (file bytes, offset) pair: the JPEG whose SOI is at that offset, decoded as CimgDecode.decode(offset=...)
+        decodes it (its scan runs to the end of the file, and its MCU file map holds absolute positions)."""
         sets, keys, descs, chunks, off = [], {}, [], [], 0
         for j in jpegs:
-            t, d, start = parse_jpeg(j)
+            j, at = j if isinstance(j, tuple) else (j, 0)
+            t, d, start = parse_jpeg(j, at)
             k = tables_key(t)
             if k not in keys:
                 keys[k] = len(sets); sets.append(t)
@@ -326,6 +369,17 @@ class BatchDecoder:
                                            counts.ctypes.data, pos.ctypes.data, int(cap)))
         first = np.concatenate([[0], np.cumsum(counts.astype(np.int64))])
         return counts, [pos[min(first[k], cap):min(first[k + 1], cap)].copy() for k in range(len(pats))]
+
+    def find_value(self, data, start, value, length, forward=True, overlays=()):
+        """jsgpu_find_value: what CwindowBuf::BufSearch(start, value, length, forward) returns over `data` (bytes or a uint8
+        array) with `overlays` [(start, bytes), ...] applied, the last one winning: (found, position)."""
+        buf = data if isinstance(data, np.ndarray) else np.frombuffer(bytes(data), np.uint8)
+        keep = [np.frombuffer(bytes(b), np.uint8) for _, b in overlays]
+        ov = (B.jsgpu_overlay * max(len(keep), 1))(*[B.jsgpu_overlay(int(o), a.size, a.ctypes.data) for (o, _), a in zip(overlays, keep)])
+        found, pos = C.c_int(0), C.c_uint64(0)
+        self._ck(self.L.jsgpu_find_value(self.ctx, buf.ctypes.data, buf.size, start, value, length, int(forward), ov, len(keep),
+                                         C.byref(found), C.byref(pos)))
+        return bool(found.value), pos.value
 
     def scan_errors(self, i):
         """jsgpu_scan_errors of image i (only for images whose status carries JSGPU_ST_EXACT = 0x40000000)."""
