@@ -406,6 +406,17 @@ typedef struct { uint64_t start; uint64_t len; const uint8_t* data; } jsgpu_over
 int jsgpu_find_value(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, uint64_t start, uint32_t value, uint32_t len, int forward,
                      const jsgpu_overlay* overlays, uint32_t noverlays, int* found, uint64_t* found_pos);
 
+/* --- every match of a value (finding every JPEG in a file) ----------------------------------------------------------------
+ * Every p in [0, n - len] whose big-endian len (1..4) bytes equal `value`, in ascending order; overlapping matches are all
+ * reported (FF D8 FF D8 FF holds FF D8 FF twice).  For FF D8 FF the positions p >= 1 are exactly the ones a chain of
+ * CwindowBuf::BufSearch(prev, 0xFFD8FF, 3, forward) calls from 0 visits, the chain JPEGsnoop's extract-all runs.
+ * *count receives the complete count; pos receives at most `cap` positions.  The file is streamed in chunks
+ * (JSGPU_SEARCH_CHUNK_BYTES, as jsgpu_search_bytes) through the search's pinned staging buffers, each chunk uploaded once and
+ * searched, counted and listed on the device, the running count kept there.  Files of 2^32 bytes or more are refused
+ * (JSGPU_EINVAL).  The batch of the context is left untouched.  Synchronous. */
+int jsgpu_find_all(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, uint32_t value, uint32_t len, uint64_t* count, uint32_t* pos,
+                   uint64_t cap);
+
 /* Pinned host memory helpers (for callers that want true async copies). */
 void* jsgpu_host_alloc(uint64_t bytes);
 void  jsgpu_host_free(void* p);

@@ -110,7 +110,7 @@ JSGPU_SYMBOLS = [
     "jsgpu_batch_begin", "jsgpu_batch_layout", "jsgpu_batch_pools", "jsgpu_batch_upload", "jsgpu_batch_decode",
     "jsgpu_batch_download", "jsgpu_batch_stage_ms", "jsgpu_timer_start", "jsgpu_timer_stop", "jsgpu_batch_launches", "jsgpu_batch_selfsync_info", "jsgpu_batch_checksums", "jsgpu_batch_errors", "jsgpu_decode_batch_host",
     "jsgpu_host_alloc", "jsgpu_host_free", "jsgpu_host_copy_rate", "jsgpu_set_preview", "jsgpu_batch_preview", "jsgpu_batch_colour_stats", "jsgpu_batch_export", "jsgpu_set_detail", "jsgpu_batch_detail",
-    "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices", "jsgpu_search_bytes", "jsgpu_find_value"]
+    "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices", "jsgpu_search_bytes", "jsgpu_find_value", "jsgpu_find_all"]
 JSIMG_SYMBOLS = [
     "jsimg_create", "jsimg_destroy", "jsimg_config", "jsimg_set_file", "jsimg_overlay_install", "jsimg_overlay_remove_all", "jsimg_Reset", "jsimg_ResetState",
     "jsimg_SetDqtEntry", "jsimg_SetDqtTables", "jsimg_GetDqtEntry", "jsimg_SetDhtTables", "jsimg_SetDhtEntry",
@@ -178,6 +178,7 @@ def load():
     L.jsgpu_search_bytes.argtypes = [vp, vp, u64, vp, vp, u32, vp, vp, u64]
     L.jsimg_search_dqt.argtypes = [vp, vp, u64, C.c_char_p, i32, C.c_char_p]
     L.jsgpu_find_value.argtypes = [vp, vp, u64, u64, u32, u32, i32, vp, u32, C.POINTER(i32), C.POINTER(u64)]
+    L.jsgpu_find_all.argtypes = [vp, vp, u64, u32, u32, C.POINTER(u64), vp, u64]
     L.jsimg_buf_search.argtypes = [vp, u64, u32, u32, i32, C.POINTER(u64)]
     L.jsimg_decode_jpeg_at.argtypes = [vp, vp, u64, u64, i32]
     L.jsimg_img_search.argtypes = [vp, u64, i32, i32, C.POINTER(i32), C.POINTER(u64), C.POINTER(i32)]

@@ -1,14 +1,76 @@
 // JfifWalk.cpp — the slice of CjfifDecode::DecodeMarker that feeds the scan decoder: walk
 // SOI / DQT / SOF0-1 / DHT / DRI / SOS and make the SAME setter calls, in the same order and with
 // the same arguments, that the reference parser makes (source/JfifDecode.cpp: DQT 4576-4651,
-// SOF 5001-5026, DHT 3535-3600, DRI 5310-5330, SOS 5150-5164 + 5291).  Everything else the
-// reference parser does (EXIF, signatures, thumbnails, logging) is out of scope (SURVEY.md §8f N1).
+// SOF 5001-5026, DHT 3535-3600, DRI 5310-5330, SOS 5150-5164 + 5291, the AVI1 Huffman-table
+// import 4406-4426).  Everything else the reference parser does (EXIF, signatures, thumbnails,
+// logging) is out of scope (SURVEY.md §8f N1).
+#include <vector>
 #include "ImgDecode.h"
 #include "JfifWalk.h"
+#include "../annex_k.h"
 
 const unsigned kJfifZigZag[64] = {
      0, 1, 8,16, 9, 2, 3,10, 17,24,32,25,18,11, 4, 5, 12,19,26,33,40,48,41,34, 27,20,13, 6, 7,14,21,28,
     35,42,49,56,57,50,43,36, 29,22,15,23,30,37,44,51, 58,59,52,45,38,31,39,46, 53,60,61,54,47,55,62,63 };
+
+// The tables of one DHT segment, [q, e): canonical codes in the reference's SetDhtEntry / SetDhtSize calls (:3535-3600).
+static int WalkDht(CimgDecode* pImgDec, const uint8_t* d, uint64_t q, uint64_t e)
+{
+    while (q < e) {
+        unsigned Tc = d[q] >> 4, Th = d[q] & 15; q++;
+        if (q + 16 > e) return JFIFWALK_ETRUNC;
+        unsigned Li[17], tot = 0;
+        for (unsigned i = 1; i <= 16; i++) { Li[i] = d[q++]; tot += Li[i]; }
+        if (q + tot > e) return JFIFWALK_ETRUNC;
+        const uint8_t* vals = d + q; q += tot;
+        unsigned nCodeVal = 0, nDhtInd = 0, nLookupInd = 0;
+        for (unsigned nBitLen = 1; nBitLen <= 16; nBitLen++) {
+            for (unsigned j = 0; j < Li[nBitLen]; j++) {
+                unsigned nMask = (unsigned)((((uint64_t)1 << nBitLen) - 1) << (32 - nBitLen));
+                pImgDec->SetDhtEntry(Th, Tc, nLookupInd, nBitLen, nCodeVal << (32 - nBitLen), nMask, vals[nDhtInd]);   // :3581
+                nLookupInd++; nCodeVal++; nDhtInd++;
+            }
+            nCodeVal <<= 1;
+        }
+        pImgDec->SetDhtSize(Th, Tc, nLookupInd);                             // :3600
+    }
+    return 0;
+}
+
+// The tables of the DHT segment a Motion-JPEG frame leaves out (OpenDML AVI, "Proposed Data Chunk Format"): the T.81
+// Annex K tables in the order DC 0, DC 1, AC 0, AC 1, as the Tc/Th bytes, BITS and HUFFVAL of one DHT segment.
+static const std::vector<uint8_t>& MjpgDhtTables()
+{
+    static const std::vector<uint8_t> seg = [] {
+        using namespace annex_k;
+        std::vector<uint8_t> s;
+        auto put = [&](uint8_t tcth, const uint8_t* bits, const uint8_t* vals, unsigned nvals) {
+            s.push_back(tcth); s.insert(s.end(), bits, bits + 16); s.insert(s.end(), vals, vals + nvals);
+        };
+        put(0x00, kDcLumBits, kDcVals, 12); put(0x01, kDcChrBits, kDcVals, 12);
+        put(0x10, kAcLumBits, kAcLumVals, 162); put(0x11, kAcChrBits, kAcChrVals, 162);
+        return s;
+    }();
+    return seg;
+}
+
+// CjfifDecode reads the APP0 identifier with BufReadStrn (WindowBuf.cpp:984-1007) from just after the length field, whatever
+// the length: up to 255 bytes, stopping at a 0 byte and keeping only printable ones, bytes past the end of the file reading
+// as 0.  A Motion-JPEG frame is one whose identifier starts with "AVI1" (JfifDecode.cpp:4406).
+static bool App0IsAvi1(const uint8_t* d, uint64_t n, uint64_t q)
+{
+    static const char kAvi1[4] = {'A', 'V', 'I', '1'};
+    unsigned k = 0;
+    for (uint64_t i = 0; i < 255 && k < 4; i++) {
+        const uint8_t c = q + i < n ? d[q + i] : 0;
+        if (c == 0) break;
+        if (c >= 0x20 && c <= 0x7E) {
+            if (c != (uint8_t)kAvi1[k]) return false;
+            k++;
+        }
+    }
+    return k == 4;
+}
 
 int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n, uint64_t nPosStart, bool* pbSof)
 {
@@ -58,24 +120,14 @@ int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n, uint64_t nPosSta
         case 0xC2: case 0xC3: case 0xC5: case 0xC6: case 0xC7: case 0xC9: case 0xCA: case 0xCB: case 0xCD: case 0xCE: case 0xCF:
             *pbSof = true;                                          // the reference parses these frames too (:4800-4812)
             return JFIFWALK_EUNSUP;
-        case 0xC4:                                                  // DHT
-            while (q < e) {
-                unsigned Tc = d[q] >> 4, Th = d[q] & 15; q++;
-                if (q + 16 > e) return JFIFWALK_ETRUNC;
-                unsigned Li[17], tot = 0;
-                for (unsigned i = 1; i <= 16; i++) { Li[i] = d[q++]; tot += Li[i]; }
-                if (q + tot > e) return JFIFWALK_ETRUNC;
-                const uint8_t* vals = d + q; q += tot;
-                unsigned nCodeVal = 0, nDhtInd = 0, nLookupInd = 0;
-                for (unsigned nBitLen = 1; nBitLen <= 16; nBitLen++) {          // canonical codes (:3535-3595)
-                    for (unsigned j = 0; j < Li[nBitLen]; j++) {
-                        unsigned nMask = (unsigned)((((uint64_t)1 << nBitLen) - 1) << (32 - nBitLen));
-                        pImgDec->SetDhtEntry(Th, Tc, nLookupInd, nBitLen, nCodeVal << (32 - nBitLen), nMask, vals[nDhtInd]);   // :3581
-                        nLookupInd++; nCodeVal++; nDhtInd++;
-                    }
-                    nCodeVal <<= 1;
-                }
-                pImgDec->SetDhtSize(Th, Tc, nLookupInd);                         // :3600
+        case 0xC4: {                                                // DHT
+            const int r = WalkDht(pImgDec, d, q, e);
+            if (r) return r;
+            break; }
+        case 0xE0:                                                  // APP0: a Motion-JPEG frame imports the tables it omits
+            if (App0IsAvi1(d, n, q)) {
+                const std::vector<uint8_t>& t = MjpgDhtTables();
+                WalkDht(pImgDec, t.data(), 0, t.size());
             }
             break;
         case 0xDD:                                                  // DRI (:5310-5330)

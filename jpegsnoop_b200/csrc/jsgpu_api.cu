@@ -1134,6 +1134,18 @@ int jsgpu_find_value(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, uint64_t s
                        found_pos, ctx->err);
 }
 
+int jsgpu_find_all(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, uint32_t value, uint32_t len, uint64_t* count, uint32_t* pos,
+                   uint64_t cap)
+{
+    if (!ctx) return JSGPU_EINVAL;
+    if (!count || (n && !data) || (cap && !pos) || len < 1 || len > 4)
+        return fail(ctx, JSGPU_EINVAL, "jsgpu_find_all: bad arguments (len %u, 1..4)", len);
+    if (n >> 32)
+        return fail(ctx, JSGPU_EINVAL, "jsgpu_find_all: %llu bytes: files of 2^32 bytes or more do not fit 32-bit offsets",
+                    (unsigned long long)n);
+    return js_find_all_run(&ctx->search, ctx->device, ctx->sm_count, data, n, value, len, count, pos, cap, ctx->err);
+}
+
 void* jsgpu_host_alloc(uint64_t bytes) { void* p = nullptr; if (cudaMallocHost(&p, bytes) != cudaSuccess) return nullptr; return p; }
 void  jsgpu_host_free(void* p) { if (p) cudaFreeHost(p); }
 

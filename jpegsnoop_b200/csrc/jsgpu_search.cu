@@ -18,7 +18,8 @@
 //                          anything, in file order, into a compact per-chunk list the host copies into place.
 // Device memory is two chunk buffers, the per-tile summaries and one chunk's emitted positions, whatever the file size.
 // The search has its own streams and buffers: a batch resident on the same context is not touched.
-// The first-match value search of Img Search Fwd / Rev (jsgpu_find_value, end of file) shares them.
+// The first-match value search of Img Search Fwd / Rev (jsgpu_find_value) and the every-match value search (jsgpu_find_all),
+// both at the end of the file, share them.
 #include "jsgpu_internal.h"
 #include <cstdlib>
 #include <cstring>
@@ -271,6 +272,7 @@ struct JsSearch {
     uint32_t* dres = nullptr; size_t res_cap = 0;
     uint32_t* dout = nullptr; size_t out_cap = 0;
     uint32_t* dfind = nullptr; uint32_t* hfind = nullptr;   // jsgpu_find_value: one result word per slot, device and pinned host
+    uint32_t* dfa[2] = {nullptr, nullptr}; size_t fa_cap = 0;   // jsgpu_find_all: per-CTA counts and output indices per slot
 };
 
 void js_search_free(JsSearch* s)
@@ -279,7 +281,7 @@ void js_search_free(JsSearch* s)
     cudaSetDevice(s->device);
     for (int i = 0; i < 2; i++) {
         if (s->st[i]) cudaStreamSynchronize(s->st[i]);
-        cudaFreeHost(s->pin[i]); cudaFree(s->dbuf[i]); cudaFree(s->dsum[i]); cudaFree(s->doff[i]);
+        cudaFreeHost(s->pin[i]); cudaFree(s->dbuf[i]); cudaFree(s->dsum[i]); cudaFree(s->doff[i]); cudaFree(s->dfa[i]);
         if (s->copied[i]) cudaEventDestroy(s->copied[i]);
         if (s->scanned[i]) cudaEventDestroy(s->scanned[i]);
         if (s->st[i]) cudaStreamDestroy(s->st[i]);
@@ -467,6 +469,23 @@ int js_search_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, 
 
 // Positions 0 .. npos-1 of one chunk: buf holds their npos + len - 1 bytes and is readable up to 20 bytes past the last
 // 16-byte group.  A position matches when its four bytes, little-endian and masked to len bytes, equal `pat`.
+// The match mask of positions p0 .. p0 + 15 (p0 a multiple of 16): five 32-bit loads, the windows cut by funnel shifts.
+__device__ __forceinline__ uint32_t fv_match16(const uint8_t* __restrict__ buf, uint32_t p0, uint32_t npos, uint32_t pat, uint32_t mask)
+{
+    uint32_t m = 0;
+    if (p0 < npos) {
+        const uint4 a = *(const uint4*)(buf + p0);
+        const uint32_t w[5] = {a.x, a.y, a.z, a.w, *(const uint32_t*)(buf + p0 + 16)};
+#pragma unroll
+        for (int k = 0; k < 16; k++) {
+            const uint32_t v = (k % 4) ? __funnelshift_r(w[k / 4], w[k / 4 + 1], 8 * (k % 4)) : w[k / 4];
+            if ((v & mask) == pat) m |= 1u << k;
+        }
+        if (npos - p0 < 16) m &= (1u << (npos - p0)) - 1u;
+    }
+    return m;
+}
+
 // res receives the lowest match (forward) or the highest match + 1 (reverse) if it beats what is there.
 __global__ void __launch_bounds__(FV_THREADS)
 k_find_value(const uint8_t* __restrict__ buf, uint32_t npos, uint32_t pat, uint32_t mask, int forward, uint32_t* __restrict__ res)
@@ -480,17 +499,7 @@ k_find_value(const uint8_t* __restrict__ buf, uint32_t npos, uint32_t pat, uint3
     for (uint32_t i = blockIdx.x; i < ntiles; i += gridDim.x) {
         const uint32_t t = forward ? i : ntiles - 1 - i;
         const uint32_t p0 = t * FV_TILE + 16 * tid;
-        uint32_t m = 0;
-        if (p0 < npos) {
-            const uint4 a = *(const uint4*)(buf + p0);
-            const uint32_t w[5] = {a.x, a.y, a.z, a.w, *(const uint32_t*)(buf + p0 + 16)};
-#pragma unroll
-            for (int k = 0; k < 16; k++) {
-                const uint32_t v = (k % 4) ? __funnelshift_r(w[k / 4], w[k / 4 + 1], 8 * (k % 4)) : w[k / 4];
-                if ((v & mask) == pat) m |= 1u << k;
-            }
-            if (npos - p0 < 16) m &= (1u << (npos - p0)) - 1u;
-        }
+        const uint32_t m = fv_match16(buf, p0, npos, pat, mask);
         const uint32_t vote = __ballot_sync(0xffffffffu, m != 0);
         if (vote && lane == (uint32_t)(forward ? __ffs(vote) - 1 : 31 - __clz(vote))) {
             if (forward) atomicMin(&s_best, p0 + __ffs(m) - 1);
@@ -598,5 +607,138 @@ int js_find_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, ui
         }
     }
     if (forward) *found = test(*found_pos);                  // the last position, which reads past EOF
+    return JSGPU_OK;
+}
+
+// ---- every match of a value (jsgpu_find_all, include/jsgpu.h) ----------------------------------------------------------
+// Each chunk is uploaded once and stays resident while three kernels run on it: k_find_all<false> counts the matches of
+// each CTA's run of consecutive tiles, k_find_all_scan turns the counts into output indices from the running total kept on
+// the device, and k_find_all<true> writes the positions in file order.  CTA b owns tiles [b * per, (b + 1) * per).
+template <bool EMIT>
+__global__ void __launch_bounds__(FV_THREADS)
+k_find_all(const uint8_t* __restrict__ buf, uint32_t npos, uint32_t pat, uint32_t mask, uint32_t per, uint32_t chunk_pos,
+           uint32_t* __restrict__ cta /*[2][gridDim.x]: counts, then first output index*/, uint32_t* __restrict__ out, uint64_t cap)
+{
+    __shared__ uint32_t s_w[FV_THREADS / 32];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t ntiles = (npos + FV_TILE - 1) / FV_TILE;
+    const uint32_t t0 = blockIdx.x * per, t1 = min(ntiles, t0 + per);
+    if (!EMIT) {
+        uint32_t c = 0;
+        for (uint32_t t = t0; t < t1; t++) c += __popc(fv_match16(buf, t * FV_TILE + 16 * tid, npos, pat, mask));
+        c = __reduce_add_sync(0xffffffffu, c);
+        if (lane == 0) s_w[warp] = c;
+        __syncthreads();
+        if (tid == 0) {
+            uint32_t sum = 0;
+            for (int k = 0; k < FV_THREADS / 32; k++) sum += s_w[k];
+            cta[blockIdx.x] = sum;
+        }
+        return;
+    }
+    uint32_t j = cta[gridDim.x + blockIdx.x];                // this CTA's first output index
+    if (cta[blockIdx.x] == 0 || j >= cap) return;
+    for (uint32_t t = t0; t < t1 && j < cap; t++) {
+        uint32_t m = fv_match16(buf, t * FV_TILE + 16 * tid, npos, pat, mask);
+        const uint32_t c = __popc(m);
+        uint32_t inc = c;                                     // inclusive scan over the warp, then over the warps
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, inc, d);
+            if (lane >= (uint32_t)d) inc += v;
+        }
+        __syncthreads();                                      // the previous tile is done with s_w
+        if (lane == 31) s_w[warp] = inc;
+        __syncthreads();
+        uint32_t before = 0, tot = 0;
+#pragma unroll
+        for (int k = 0; k < FV_THREADS / 32; k++) { const uint32_t v = s_w[k]; before += (uint32_t)k < warp ? v : 0u; tot += v; }
+        uint64_t o = (uint64_t)j + before + inc - c;
+        const uint32_t p = chunk_pos + t * FV_TILE + 16 * tid;
+        while (m && o < cap) { out[o++] = p + (uint32_t)__ffs((int)m) - 1; m &= m - 1; }
+        j += tot;
+    }
+}
+
+// One CTA: the first output index of every CTA of the chunk, from the running total, which it then advances.
+__global__ void __launch_bounds__(1024)
+k_find_all_scan(uint32_t* __restrict__ cta, uint32_t ncta, uint32_t* __restrict__ total)
+{
+    __shared__ uint32_t s_w[32], s_run;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) s_run = *total;
+    for (uint32_t b0 = 0; b0 < ncta; b0 += 1024) {
+        __syncthreads();
+        const uint32_t b = b0 + tid, c = b < ncta ? cta[b] : 0u;
+        uint32_t inc = c;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, inc, d);
+            if (lane >= (uint32_t)d) inc += v;
+        }
+        if (lane == 31) s_w[warp] = inc;
+        __syncthreads();
+        uint32_t before = 0, tot = 0;
+        for (uint32_t k = 0; k < 32; k++) { const uint32_t v = s_w[k]; before += k < warp ? v : 0u; tot += v; }
+        if (b < ncta) cta[ncta + b] = s_run + before + inc - c;
+        __syncthreads();
+        if (tid == 0) s_run += tot;
+    }
+    __syncthreads();
+    if (tid == 0) *total = s_run;
+}
+
+int js_find_all_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, uint64_t n, uint32_t value, uint32_t len,
+                    uint64_t* count, uint32_t* pos, uint64_t cap, std::string& err)
+{
+    *count = 0;
+    const uint32_t mask = len == 4 ? 0xFFFFFFFFu : (1u << (8 * len)) - 1u;
+    if (n < len || (value & ~mask)) return JSGPU_OK;         // no position, or a value wider than len bytes
+    SR_TRY(sr_open(ps, device, err));
+    JsSearch* s = *ps;
+    const uint64_t npos_all = n - len + 1;
+    const uint64_t chunk = std::min<uint64_t>(sr_chunk_bytes(), (npos_all + FV_TILE - 1) / FV_TILE * FV_TILE);
+    const uint64_t nchunks = (npos_all + chunk - 1) / chunk;
+    SR_TRY(sr_reserve(s, chunk + 3, chunk + 64, err));
+    int occ = 0;
+    SR_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_find_all<true>, FV_THREADS, 0));
+    const uint32_t grid_max = (uint32_t)(std::max(occ, 1) * sm_count);
+    if (s->fa_cap < 2 * (size_t)grid_max) {
+        for (int i = 0; i < 2; i++) { cudaFree(s->dfa[i]); s->dfa[i] = nullptr; }
+        s->fa_cap = 0;
+        for (int i = 0; i < 2; i++) SR_CK(cudaMalloc((void**)&s->dfa[i], 2 * (size_t)grid_max * 4));
+        s->fa_cap = 2 * (size_t)grid_max;
+    }
+    const uint64_t keep = std::min<uint64_t>(cap, npos_all);  // positions the device list can hold
+    if (keep) SR_CK(sr_grow(s->dout, s->out_cap, (size_t)keep));
+    const uint32_t pat = __builtin_bswap32(value) >> (32 - 8 * len);      // the bytes in file order, little-endian
+    uint32_t* const total = s->dfind;                                     // the running count (the value search's result word)
+    SR_CK(cudaMemsetAsync(total, 0, 4, s->st[0]));
+    SR_CK(cudaEventRecord(s->scanned[1], s->st[0]));                      // chunk 0's scan follows the reset
+
+    for (uint64_t c = 0; c < nchunks; c++) {
+        const int sl = (int)(c & 1);
+        const uint64_t plo = c * chunk;
+        const uint32_t npos = (uint32_t)std::min<uint64_t>(chunk, npos_all - plo);
+        SR_CK(cudaEventSynchronize(s->copied[sl]));           // the pinned buffer's previous upload has left
+        memcpy(s->pin[sl], data + plo, npos + len - 1);
+        SR_CK(cudaMemcpyAsync(s->dbuf[sl], s->pin[sl], npos + len - 1, cudaMemcpyHostToDevice, s->st[sl]));
+        SR_CK(cudaEventRecord(s->copied[sl], s->st[sl]));
+        const uint32_t ntiles = (npos + FV_TILE - 1) / FV_TILE;
+        const uint32_t grid = std::max(1u, std::min(grid_max, ntiles)), per = (ntiles + grid - 1) / grid;
+        k_find_all<false><<<grid, FV_THREADS, 0, s->st[sl]>>>(s->dbuf[sl], npos, pat, mask, per, (uint32_t)plo, s->dfa[sl], nullptr, 0);
+        SR_CK(cudaStreamWaitEvent(s->st[sl], s->scanned[sl ^ 1], 0));  // the previous chunk has advanced the total
+        k_find_all_scan<<<1, 1024, 0, s->st[sl]>>>(s->dfa[sl], grid, total);
+        SR_CK(cudaEventRecord(s->scanned[sl], s->st[sl]));
+        if (keep)
+            k_find_all<true><<<grid, FV_THREADS, 0, s->st[sl]>>>(s->dbuf[sl], npos, pat, mask, per, (uint32_t)plo, s->dfa[sl], s->dout, keep);
+        SR_CK(cudaGetLastError());
+    }
+    SR_CK(cudaStreamSynchronize(s->st[0])); SR_CK(cudaStreamSynchronize(s->st[1]));
+    uint32_t tot = 0;
+    SR_CK(cudaMemcpy(&tot, total, 4, cudaMemcpyDeviceToHost));
+    *count = tot;
+    const uint64_t got = std::min<uint64_t>(tot, keep);
+    if (got) SR_CK(cudaMemcpy(pos, s->dout, got * 4, cudaMemcpyDeviceToHost));
     return JSGPU_OK;
 }

@@ -232,16 +232,49 @@ class CimgDecode:
         return self._img_search(start, False, quiet)
 
 
+def _u8(data):
+    """`data` as a uint8 array, without a copy where it already is one (bytes are viewed in place)."""
+    if isinstance(data, np.ndarray) and data.dtype == np.uint8 and data.ndim == 1 and data.flags.c_contiguous:
+        return data
+    return np.frombuffer(bytes(data), np.uint8)
+
+
+def walk_jpeg(jpeg_bytes, offset=0):
+    """Marker walk from the SOI at `offset` -> (jsgpu_tables, jsgpu_image_desc, scan start, or the walk's negative error code)."""
+    buf = _u8(jpeg_bytes)
+    t = B.jsgpu_tables(); d = B.jsgpu_image_desc()
+    r = B.load().jsimg_parse_jpeg_at(buf.ctypes.data, buf.size, offset, C.byref(t), C.byref(d))
+    return t, d, r
+
+
 def parse_jpeg(jpeg_bytes, offset=0):
     """Marker walk only, from the SOI at `offset` -> (jsgpu_tables, jsgpu_image_desc, scan_start); the scan start and
     desc.file_pos are absolute offsets in `jpeg_bytes`."""
-    L = B.load()
-    buf = np.frombuffer(bytes(jpeg_bytes), np.uint8)
-    t = B.jsgpu_tables(); d = B.jsgpu_image_desc()
-    r = L.jsimg_parse_jpeg_at(buf.ctypes.data, buf.size, offset, C.byref(t), C.byref(d))
+    t, d, r = walk_jpeg(jpeg_bytes, offset)
     if r < 0:
         raise ValueError(f"marker walk failed ({r}) at offset {offset}")
     return t, d, r
+
+
+SOI3 = 0xFFD8FF
+WINDOW_SLACK = 64     # bytes a scan window reads past the next SOI candidate; an accepted scan ends at least this far inside it
+
+
+def plan_windows(data, candidates):
+    """The first pass of BatchDecoder.decode_all: for every SOI candidate p (ascending) -> (p, scan start or the walk's error
+    code, window end w).  A walked image reads [scan start, w), w = min(n, q + WINDOW_SLACK) with q the first candidate past
+    its scan start (FF D8 is a marker, so a healthy scan ends by q); w is None for a failed walk."""
+    buf = _u8(data)
+    cands = np.asarray(candidates, np.int64)
+    out = []
+    for p in cands.tolist():
+        _, _, r = walk_jpeg(buf, p)
+        if r < 0:
+            out.append((p, r, None))
+            continue
+        k = int(np.searchsorted(cands, r, side="right"))
+        out.append((p, r, buf.size if k == cands.size else min(buf.size, int(cands[k]) + WINDOW_SLACK)))
+    return out
 
 
 def tables_key(t):
@@ -302,16 +335,21 @@ class BatchDecoder:
         """Host-side preparation: marker walk of every JPEG, table-set dedupe, concatenation of the
         scan bytes.  Returns (table_sets array, descs array, bitstream uint8 array).  An entry may be a
         (file bytes, offset) pair: the JPEG whose SOI is at that offset, decoded as CimgDecode.decode(offset=...)
-        decodes it (its scan runs to the end of the file, and its MCU file map holds absolute positions)."""
+        decodes it (its scan runs to the end of the file, and its MCU file map holds absolute positions).
+        An (file bytes, offset, length) triple reads the file as if it ended at offset + length: only the scan bytes
+        before that point are copied, and positions stay absolute."""
         sets, keys, descs, chunks, off = [], {}, [], [], 0
         for j in jpegs:
-            j, at = j if isinstance(j, tuple) else (j, 0)
+            j, at, *length = j if isinstance(j, tuple) else (j, 0)
+            j = _u8(j)
+            if length:
+                j = j[:at + length[0]]
             t, d, start = parse_jpeg(j, at)
             k = tables_key(t)
             if k not in keys:
                 keys[k] = len(sets); sets.append(t)
             d.table_set = keys[k]
-            scan = np.frombuffer(bytes(j), np.uint8)[start:]
+            scan = j[start:]
             d.scan_offset = off; d.scan_length = scan.size; d.file_pos = start
             chunks.append(scan); off += (scan.size + 15) // 16 * 16
             descs.append(d)
@@ -380,6 +418,64 @@ class BatchDecoder:
         self._ck(self.L.jsgpu_find_value(self.ctx, buf.ctypes.data, buf.size, start, value, length, int(forward), ov, len(keep),
                                          C.byref(found), C.byref(pos)))
         return bool(found.value), pos.value
+
+    def find_all(self, data, value=SOI3, length=3, cap=None):
+        """jsgpu_find_all: every position of the big-endian `length`-byte `value` in `data` (bytes or a uint8 array), overlapping
+        ones included -> (count, positions uint32 ascending).  With `cap`, at most cap positions are returned (count stays
+        complete); without it, all of them (a second pass runs only when there are more than one per 2 KiB of file)."""
+        buf = _u8(data)
+        count = C.c_uint64(0)
+        want = cap if cap is not None else buf.size // 2048 + 1024
+        pos = np.zeros(max(int(want), 1), np.uint32)
+        self._ck(self.L.jsgpu_find_all(self.ctx, buf.ctypes.data, buf.size, value, length, C.byref(count), pos.ctypes.data, int(want)))
+        if cap is None and count.value > want:
+            want = count.value; pos = np.zeros(want, np.uint32)
+            self._ck(self.L.jsgpu_find_all(self.ctx, buf.ctypes.data, buf.size, value, length, C.byref(count), pos.ctypes.data, want))
+        return int(count.value), pos[:min(int(count.value), int(want))]
+
+    def decode_all(self, data, redo_budget=1 << 30):
+        """Every JPEG in `data` in one batch: the SOI candidates of find_all(), each walked from its offset, each walked image
+        decoded from a window of its scan (plan_windows), so that a file of K images uploads about its own size rather than
+        K times it.  An image keeps its windowed outputs when its window runs to the end of the file, or when it decoded
+        without error and the marker ending its scan lies at least WINDOW_SLACK bytes inside the window; every other image is
+        decoded again from its scan start to the end of the file, as the reference reads a damaged scan on through markers,
+        in batches of at most `redo_budget` scan bytes (an image longer than that alone).
+        Returns ([(offset, scan start or the walk's error code, DecodedImage or None)] in file order,
+                 {"redone": images decoded again, "uploaded": bitstream bytes uploaded in all}).
+        Every image equals CimgDecode.decode(data, offset=p) but for nerr: positions absolute, status included."""
+        buf = _u8(data)
+        n = buf.size
+        _, cands = self.find_all(buf)
+        plan = plan_windows(buf, cands)
+        imgs = [None] * len(plan)
+        walked = [k for k, (_, r, _) in enumerate(plan) if r >= 0]
+        uploaded = 0
+
+        def run(entries, ks, accept):
+            nonlocal uploaded
+            tarr, darr, bits = self.prepare(entries)
+            self.set_tables(tarr); self.plan(darr, bits.size); self.upload(bits); self.decode(); self.sync()
+            uploaded += bits.size
+            self.refresh_layout()
+            for i, k in enumerate(ks):
+                d = self.fetch(i, refresh=False)
+                d.pos, d.scan_start = plan[k][0], plan[k][1]
+                if accept(d, plan[k][2]):
+                    imgs[k] = d
+
+        if walked:
+            run([(buf, plan[k][0], plan[k][2] - plan[k][0]) for k in walked], walked,
+                lambda d, w: w == n or (d.status == 0 and d.scan_start <= (int(d.stats[14]) & 0xFFFFFFFF) <= w - WINDOW_SLACK))
+        redo = [k for k in walked if imgs[k] is None]
+        group, size = [], 0
+        for k in redo + [None]:
+            tail = None if k is None else n - plan[k][1]
+            if group and (k is None or size + tail > redo_budget):
+                run([(buf, plan[g][0]) for g in group], group, lambda d, w: True)
+                group, size = [], 0
+            if k is not None:
+                group.append(k); size += tail
+        return [(p, r, imgs[k]) for k, (p, r, _) in enumerate(plan)], {"redone": len(redo), "uploaded": uploaded}
 
     def scan_errors(self, i):
         """jsgpu_scan_errors of image i (only for images whose status carries JSGPU_ST_EXACT = 0x40000000)."""
@@ -472,9 +568,10 @@ class BatchDecoder:
                 ("mcu_map", B.OUT_MCU_MAP, np.uint32, (nmcu,), int(lo.mcu_off), False),
                 ("dht_histo", B.OUT_HISTO, np.uint32, (2, 4, 17), i * 136, False), ("stats", B.OUT_STATS, np.int32, (16,), i * 16, False)]
 
-    def _image(self, i, get):
+    def _image(self, i, get, refresh=True):
         """DecodedImage of image i, each output from get(name, selector, dtype, shape, offset)."""
-        self.refresh_layout()
+        if refresh:
+            self.refresh_layout()
         lo = self.layout[i]; d = DecodedImage()
         d.geom = np.array([lo.mcu_w, lo.mcu_h, lo.mcu_xmax, lo.mcu_ymax, lo.blk_xmax, lo.blk_ymax, lo.img_x, lo.img_y], np.uint32)
         ns = self.descs[i].num_sos_comps
@@ -489,8 +586,9 @@ class BatchDecoder:
         """The same DecodedImage as fetch(), cut out of the host buffers a decode_host() call filled."""
         return self._image(i, lambda name, sel, dtype, shape, off: np.array(outs[name][off:off + int(np.prod(shape))]).reshape(shape))
 
-    def fetch(self, i):
+    def fetch(self, i, refresh=True):
+        """DecodedImage of image i; refresh=False reuses the layout read after the last decode (one read for a whole batch)."""
         def dl(name, sel, dtype, shape, off):
             a = np.zeros(shape, dtype)
             self._ck(self.L.jsgpu_batch_download(self.ctx, sel, i, a.ctypes.data, a.nbytes)); return a
-        return self._image(i, dl)
+        return self._image(i, dl, refresh)
