@@ -103,8 +103,8 @@ typedef struct {
     int32_t want_histo;     /* accumulate m_anDhtHisto (ImgDecode.cpp:1190-1191); default 1      */
     int32_t want_mcu_map;   /* build m_pMcuFileMap (ImgDecode.cpp:3229); default 1               */
     int32_t device_markers; /* ignored: RSTn and the end of scan are always found on the GPU      */
-    int32_t scan_err_max;   /* CSnoopConfig::nErrMaxDecodeScan (SnoopConfig.cpp:89): capped error lines
-                               per scan; 0 = the reference's default, 20                          */
+    uint32_t scan_err_max;  /* CSnoopConfig::nErrMaxDecodeScan (SnoopConfig.cpp:89), taken literally: the capped error lines of
+                               a scan are reported while fewer than this many were (0: none at all); jsgpu_init sets 20   */
 } jsgpu_options;
 
 /* Device pointers of the output pools of the current batch (owned by the context). */
@@ -169,6 +169,11 @@ int  jsgpu_sync(jsgpu_ctx* ctx);
 int jsgpu_set_idct_tables(jsgpu_ctx* ctx, const int32_t* li, const float* lf);
 int jsgpu_set_options(jsgpu_ctx* ctx, const jsgpu_options* opt);
 int jsgpu_get_options(jsgpu_ctx* ctx, jsgpu_options* opt);
+/* The error report's state when the next decode's scans start (jsgpu_init: 0, 0): warn_start = m_nWarnBadScanNum, the capped
+ * lines already counted (the cap after ScanErrorsDisable, ImgDecode.cpp:1014-1018, which Reset() keeps, :127); disable =
+ * m_bScanErrorsDisable, which drops the uncapped "Expected RST marker index" line (:1417).  Each scan's final count comes back
+ * in jsgpu_scan_errors.warn_num. */
+int jsgpu_set_scan_error_state(jsgpu_ctx* ctx, uint32_t warn_start, int disable);
 /* Replaces SetDqtEntry / SetDhtEntry / SetDhtSize state (ImgDecode.cpp:424-453,748-847):
  * builds the device look-up tables for `nsets` table sets. */
 int jsgpu_upload_tables(jsgpu_ctx* ctx, const jsgpu_tables* sets, uint32_t nsets);
@@ -245,12 +250,16 @@ typedef struct {
     uint32_t restart_read;    /* m_nRestartRead                                                                           */
     uint32_t done;
     uint32_t end_pos, end_align;  /* m_anScanBuffPtr_pos[0], m_nScanBuffPtr_align after the last MCU */
-    uint32_t pad;
+    uint32_t warn_num;        /* m_nWarnBadScanNum after the scan: scan_warn_start plus the capped lines counted              */
     jsgpu_scan_event ev[JSGPU_MAX_EVENTS];
 } jsgpu_scan_errors;
 /* Error events of image `image` of the last decode (JSGPU_ESTATE when it did not take the serial path: status without
- * JSGPU_ST_EXACT).  Forces a sync. */
+ * JSGPU_ST_EXACT).  The counts are complete; ev[] holds the first JSGPU_MAX_EVENTS events.  Forces a sync. */
 int jsgpu_batch_errors(jsgpu_ctx* ctx, uint32_t image, jsgpu_scan_errors* out);
+/* Events first .. first+n-1 of all nevents of that image (n * 32 bytes); JSGPU_EINVAL past nevents.  Events past the first
+ * JSGPU_MAX_EVENTS come from a second, events-only walk of the image over the resident scan, with the decode's cap, start
+ * count and disable flag: it writes no output and gives the same events.  Forces a sync. */
+int jsgpu_batch_error_events(jsgpu_ctx* ctx, uint32_t image, uint32_t first, uint32_t n, jsgpu_scan_event* out);
 
 /* Checksums of the outputs of every image of the last jsgpu_batch_decode, computed on the device (forces a sync):
  * ck[i][0..2] m_pPixValY/Cb/Cr, [3] the DIB, [4..6] m_pBlkDcValY/Cb/Cr, [7] m_pMcuFileMap, [8] m_anDhtHisto, [9] the nine

@@ -22,6 +22,14 @@ void   jsimg_destroy(jsimg*);
 void   jsimg_config(jsimg*, int decode_ac, int idct_fixedpt, int cuda_device, int huff_kernel, int idct_kernel, int device_markers);
 /* CSnoopConfig::bHistoEn / bStatClipEn / bDumpHistoY (SnoopConfig.cpp:76-82), read at ImgDecode.cpp:2730-2741 */
 void   jsimg_config_histo(jsimg*, int histo_en, int statclip_en, int dump_histo_y);
+/* CSnoopConfig::nErrMaxDecodeScan (SnoopConfig.cpp:89, default 20), read at ImgDecode.cpp:2732: each kind of capped scan
+ * error line is reported while fewer than n were; 0 reports none of them */
+void   jsimg_config_scan_err_max(jsimg*, unsigned n);
+/* CimgDecode::ScanErrorsDisable / ScanErrorsEnable (ImgDecode.cpp:1014-1030): disabling counts the cap as used up (the count
+ * survives Reset(), so a cap raised later lets only the difference through) and drops the "Expected RST marker index" lines;
+ * enabling sets the count back to 0.  ResetState() (every marker walk) clears the switch. */
+void   jsimg_ScanErrorsDisable(jsimg*);
+void   jsimg_ScanErrorsEnable(jsimg*);
 /* byte source: CwindowBuf::BufFileSet equivalent on a memory buffer (caller keeps it alive) */
 void   jsimg_set_file(jsimg*, const uint8_t* data, uint64_t n);
 int    jsimg_overlay_install(jsimg*, uint32_t start, const uint8_t* data, uint32_t n);

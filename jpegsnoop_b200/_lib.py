@@ -43,7 +43,7 @@ class jsgpu_image_layout(C.Structure):
 class jsgpu_options(C.Structure):
     _fields_ = [("idct_mode", C.c_int32), ("decode_ac", C.c_int32), ("huff_kernel", C.c_int32),
                 ("idct_kernel", C.c_int32), ("want_histo", C.c_int32), ("want_mcu_map", C.c_int32),
-                ("device_markers", C.c_int32), ("scan_err_max", C.c_int32)]
+                ("device_markers", C.c_int32), ("scan_err_max", C.c_uint32)]
 
 
 class jsgpu_scan_event(C.Structure):
@@ -52,7 +52,7 @@ class jsgpu_scan_event(C.Structure):
 
 class jsgpu_scan_errors(C.Structure):
     _fields_ = [("nerr_lines", C.c_uint32), ("nevents", C.c_uint32), ("scan_bad", C.c_uint32), ("restart_read", C.c_uint32),
-                ("done", C.c_uint32), ("end_pos", C.c_uint32), ("end_align", C.c_uint32), ("pad", C.c_uint32), ("ev", jsgpu_scan_event * 256)]
+                ("done", C.c_uint32), ("end_pos", C.c_uint32), ("end_align", C.c_uint32), ("warn_num", C.c_uint32), ("ev", jsgpu_scan_event * 256)]
 
 
 class jsgpu_pools(C.Structure):
@@ -106,9 +106,9 @@ OUT_PIX_Y, OUT_PIX_CB, OUT_PIX_CR, OUT_DIB, OUT_BLK_Y, OUT_BLK_CB, OUT_BLK_CR, O
 # every symbol include/jsgpu.h and include/jsimg.h declare (tests check they are all exported)
 JSGPU_SYMBOLS = [
     "jsgpu_init", "jsgpu_free", "jsgpu_last_error", "jsgpu_strerror", "jsgpu_version", "jsgpu_stream", "jsgpu_sync",
-    "jsgpu_set_idct_tables", "jsgpu_set_options", "jsgpu_get_options", "jsgpu_upload_tables", "jsgpu_bcast_tables",
+    "jsgpu_set_idct_tables", "jsgpu_set_options", "jsgpu_get_options", "jsgpu_set_scan_error_state", "jsgpu_upload_tables", "jsgpu_bcast_tables",
     "jsgpu_batch_begin", "jsgpu_batch_layout", "jsgpu_batch_pools", "jsgpu_batch_upload", "jsgpu_batch_decode",
-    "jsgpu_batch_download", "jsgpu_batch_stage_ms", "jsgpu_timer_start", "jsgpu_timer_stop", "jsgpu_batch_launches", "jsgpu_batch_selfsync_info", "jsgpu_batch_checksums", "jsgpu_batch_errors", "jsgpu_decode_batch_host",
+    "jsgpu_batch_download", "jsgpu_batch_stage_ms", "jsgpu_timer_start", "jsgpu_timer_stop", "jsgpu_batch_launches", "jsgpu_batch_selfsync_info", "jsgpu_batch_checksums", "jsgpu_batch_errors", "jsgpu_batch_error_events", "jsgpu_decode_batch_host",
     "jsgpu_host_alloc", "jsgpu_host_free", "jsgpu_host_copy_rate", "jsgpu_set_preview", "jsgpu_batch_preview", "jsgpu_batch_colour_stats", "jsgpu_batch_export", "jsgpu_set_detail", "jsgpu_batch_detail",
     "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices", "jsgpu_search_bytes", "jsgpu_find_value", "jsgpu_find_all"]
 JSIMG_SYMBOLS = [
@@ -121,7 +121,8 @@ JSIMG_SYMBOLS = [
     "jsimg_log_count", "jsimg_log_line", "jsimg_log_clear", "jsimg_walk_jpeg", "jsimg_decode_jpeg", "jsimg_parse_jpeg",
     "jsimg_config_histo", "jsimg_SetPreviewMode", "jsimg_GetPreviewMode", "jsimg_SetPreviewYccOffset", "jsimg_GetPreviewYccOffset",
     "jsimg_GetStatClip", "jsimg_GetHistoRanges", "jsimg_GetCcHisto", "jsimg_GetHistoYFull", "jsimg_GetHistoDib", "jsimg_ExportTiff", "jsimg_tiff_write", "jsimg_SetDetailVlc", "jsimg_GetDetailVlc",
-    "jsimg_search_dqt", "jsimg_buf_search", "jsimg_decode_jpeg_at", "jsimg_img_search", "jsimg_decode_offset_mode", "jsimg_parse_jpeg_at"]
+    "jsimg_search_dqt", "jsimg_buf_search", "jsimg_decode_jpeg_at", "jsimg_img_search", "jsimg_decode_offset_mode", "jsimg_parse_jpeg_at",
+    "jsimg_config_scan_err_max", "jsimg_ScanErrorsDisable", "jsimg_ScanErrorsEnable"]
 
 _lib = None
 
@@ -145,6 +146,7 @@ def load():
     L.jsgpu_set_idct_tables.argtypes = [vp, vp, vp]
     L.jsgpu_set_options.argtypes = [vp, C.POINTER(jsgpu_options)]
     L.jsgpu_get_options.argtypes = [vp, C.POINTER(jsgpu_options)]
+    L.jsgpu_set_scan_error_state.argtypes = [vp, u32, i32]
     L.jsgpu_upload_tables.argtypes = [vp, vp, u32]
     L.jsgpu_bcast_tables.argtypes = [vp, vp, u32, vp, i32]
     L.jsgpu_batch_begin.argtypes = [vp, vp, u32, u64]
@@ -158,6 +160,7 @@ def load():
     L.jsgpu_batch_selfsync_info.argtypes = [vp, vp, u32]
     L.jsgpu_batch_checksums.argtypes = [vp, vp, u32]
     L.jsgpu_batch_errors.argtypes = [vp, u32, C.POINTER(jsgpu_scan_errors)]
+    L.jsgpu_batch_error_events.argtypes = [vp, u32, u32, u32, vp]
     L.jsgpu_timer_start.argtypes = [vp]
     L.jsgpu_timer_stop.argtypes = [vp, C.POINTER(C.c_float)]
     L.jsgpu_decode_batch_host.argtypes = [vp, vp, u32, vp, u64, C.POINTER(jsgpu_host_outputs)]
@@ -187,6 +190,9 @@ def load():
     L.jsimg_SetDetailVlc.argtypes = [vp, i32, u32, u32, u32]; L.jsimg_SetDetailVlc.restype = None
     L.jsimg_GetDetailVlc.argtypes = [vp] + [C.POINTER(u32)] * 4; L.jsimg_GetDetailVlc.restype = None
     L.jsimg_config_histo.argtypes = [vp, i32, i32, i32]; L.jsimg_config_histo.restype = None
+    L.jsimg_config_scan_err_max.argtypes = [vp, u32]; L.jsimg_config_scan_err_max.restype = None
+    for n in ("jsimg_ScanErrorsDisable", "jsimg_ScanErrorsEnable"):
+        getattr(L, n).argtypes = [vp]; getattr(L, n).restype = None
     L.jsimg_SetPreviewMode.argtypes = [vp, u32]; L.jsimg_SetPreviewMode.restype = None
     L.jsimg_GetPreviewMode.argtypes = [vp]; L.jsimg_GetPreviewMode.restype = u32
     L.jsimg_SetPreviewYccOffset.argtypes = [vp, u32, u32, i32, i32, i32]; L.jsimg_SetPreviewYccOffset.restype = None

@@ -344,8 +344,9 @@ void CimgDecode::DecodeScanImg(unsigned nStart, bool bDisplay, bool bQuiet)
     opt.decode_ac = m_bDecodeScanAc ? 1 : 0;
     opt.huff_kernel = JS_CFG_HUFF(m_pAppConfig); opt.idct_kernel = JS_CFG_IDCTK(m_pAppConfig);
     opt.want_histo = 1; opt.want_mcu_map = 1;
-    opt.scan_err_max = (int32_t)m_nScanErrMax;
+    opt.scan_err_max = m_nScanErrMax;
     jsgpu_set_options(m_pGpu, &opt);
+    jsgpu_set_scan_error_state(m_pGpu, m_nWarnBadScanNum, m_bScanErrorsDisable ? 1 : 0);
     // CalcChannelPreview() at the end of the decode (ref :3641-3643) with this object's preview settings: the device takes the
     // extra colour pass inside jsgpu_batch_decode only when they differ from the defaults
     jsgpu_preview pv; PreviewSettings(pv);
@@ -383,7 +384,15 @@ void CimgDecode::DecodeScanImg(unsigned nStart, bool bDisplay, bool bQuiet)
     jsgpu_batch_stage_ms(m_pGpu, m_afStageMs);
     jsgpu_batch_download(m_pGpu, JSGPU_OUT_MCU_MAP, 0, m_pMcuFileMap, nMcu * 4);
     jsgpu_batch_download(m_pGpu, JSGPU_OUT_BLK_Y, 0, m_pBlkDcValY, nBlk * 2);
-    jsgpu_batch_download(m_pGpu, JSGPU_OUT_HISTO, 0, m_anDhtHisto, sizeof m_anDhtHisto);
+    {
+        // the reference counts into m_anDhtHisto (ref :1191) and clears it only in ResetDhtLookup (ref :375): a second
+        // DecodeScanImg without a new marker walk adds to the first one's counts
+        unsigned anHisto[JSGPU_HISTO_WORDS];
+        jsgpu_batch_download(m_pGpu, JSGPU_OUT_HISTO, 0, anHisto, sizeof anHisto);
+        static_assert(sizeof anHisto == sizeof m_anDhtHisto, "histogram layout");
+        unsigned* pHisto = &m_anDhtHisto[0][0][0];
+        for (unsigned i = 0; i < JSGPU_HISTO_WORDS; i++) pHisto[i] += anHisto[i];
+    }
     if (m_nNumSosComps == NUM_CHAN_YCC) {
         jsgpu_batch_download(m_pGpu, JSGPU_OUT_BLK_CB, 0, m_pBlkDcValCb, nBlk * 2);
         jsgpu_batch_download(m_pGpu, JSGPU_OUT_BLK_CR, 0, m_pBlkDcValCr, nBlk * 2);
@@ -417,7 +426,19 @@ void CimgDecode::DecodeScanImg(unsigned nStart, bool bDisplay, bool bQuiet)
         const bool bExact = (lo.status & JSGPU_ST_EXACT) != 0;
         const bool bHaveDet = m_bDetailVlc && jsgpu_batch_detail_info(m_pGpu, anDetInfo) == JSGPU_OK;
         const bool bHaveErr = (bExact || bHaveDet) && jsgpu_batch_errors(m_pGpu, 0, pErr) == JSGPU_OK;
-        const unsigned nEv = bHaveErr ? (pErr->nevents < JSGPU_MAX_EVENTS ? pErr->nevents : JSGPU_MAX_EVENTS) : 0;
+        // every event: the first JSGPU_MAX_EVENTS came with pErr, the rest from an events-only walk on the device
+        std::vector<jsgpu_scan_event> vErr;
+        if (bHaveErr) {
+            vErr.assign(pErr->ev, pErr->ev + (pErr->nevents < JSGPU_MAX_EVENTS ? pErr->nevents : JSGPU_MAX_EVENTS));
+            if (pErr->nevents > JSGPU_MAX_EVENTS) {
+                vErr.resize(pErr->nevents);
+                if (jsgpu_batch_error_events(m_pGpu, 0, 0, pErr->nevents, vErr.data()) != JSGPU_OK) {
+                    vErr.resize(JSGPU_MAX_EVENTS);
+                    m_pLog->AddLineErr(JS_LOGSTR(fmt("*** ERROR: GPU scan decoder: error events past the first %u unavailable: %s ***", JSGPU_MAX_EVENTS, jsgpu_last_error(m_pGpu))));
+                }
+            }
+        }
+        const unsigned nEv = (unsigned)vErr.size();
         unsigned iEv = 0;
         if (bHaveDet) {
             // every event and matrix, read in pages (the matrices in the order the events name them)
@@ -430,7 +451,7 @@ void CimgDecode::DecodeScanImg(unsigned nStart, bool bDisplay, bool bQuiet)
                 if (jsgpu_batch_detail_events(m_pGpu, nFirst, n, vEv.data()) != JSGPU_OK) break;
                 for (unsigned i = 0; i < n; i++) {
                     const jsgpu_detail_event& e = vEv[i];
-                    for (; iEv < nEv && iEv < e.seq; iEv++) { if (pErr->ev[iEv].code == JSGPU_EV_MARKER_NOTE) bMarkerNoteLogged = true; LogScanEvent(pErr->ev[iEv]); }
+                    for (; iEv < nEv && iEv < e.seq; iEv++) { if (vErr[iEv].code == JSGPU_EV_MARKER_NOTE) bMarkerNoteLogged = true; LogScanEvent(vErr[iEv]); }
                     const int16_t* pMat = nullptr;
                     if (e.kind == JSGPU_DT_MATRIX && e.a < nBlk) {
                         if (e.a < nMatFirst || e.a >= nMatFirst + nMatHave) {
@@ -446,10 +467,9 @@ void CimgDecode::DecodeScanImg(unsigned nStart, bool bDisplay, bool bQuiet)
         if (bExact) {
             if (bHaveErr) {
                 m_bScanBad = pErr->scan_bad != 0;
-                for (; iEv < nEv; iEv++) LogScanEvent(pErr->ev[iEv]);
-                if (pErr->nevents > JSGPU_MAX_EVENTS)
-                    m_pLog->AddLineErr(JS_LOGSTR(fmt("    (%u further scan error events not itemised)", pErr->nevents - JSGPU_MAX_EVENTS)));
+                for (; iEv < nEv; iEv++) LogScanEvent(vErr[iEv]);
                 m_nRestartRead = pErr->restart_read;
+                m_nWarnBadScanNum = pErr->warn_num;                 // what the walk counted: kept across decodes while errors are disabled
             } else {
                 m_bScanBad = true;
                 m_pLog->AddLineErr(JS_LOGSTR(fmt("*** ERROR: Bad scan data (device status 0x%08X; error events unavailable: %s) ***", lo.status, jsgpu_last_error(m_pGpu))));
@@ -457,7 +477,7 @@ void CimgDecode::DecodeScanImg(unsigned nStart, bool bDisplay, bool bQuiet)
         } else {
             // a healthy image walked only for its detailed decode: the walk stops after the printed MCUs; what it met up to there
             // (the end-of-scan marker, when the range reaches the end of the image) has its place among the dump lines
-            for (; iEv < nEv; iEv++) { if (pErr->ev[iEv].code == JSGPU_EV_MARKER_NOTE) bMarkerNoteLogged = true; LogScanEvent(pErr->ev[iEv]); }
+            for (; iEv < nEv; iEv++) { if (vErr[iEv].code == JSGPU_EV_MARKER_NOTE) bMarkerNoteLogged = true; LogScanEvent(vErr[iEv]); }
             if (lo.status) { m_bScanBad = true; m_pLog->AddLineErr(JS_LOGSTR(fmt("*** ERROR: Bad scan data (device status 0x%08X) ***", lo.status))); }
         }
         delete pErr;

@@ -18,6 +18,9 @@ jsimg* jsimg_create(void) { return new jsimg(); }
 void jsimg_destroy(jsimg* h) { delete h; }
 void jsimg_config(jsimg* h, int ac, int fixed, int dev, int hk, int ik, int)
 { h->cfg.bDecodeScanImgAc = ac != 0; h->cfg.bIdctFixedPt = fixed != 0; h->cfg.nCudaDevice = dev; h->cfg.nHuffKernel = hk; h->cfg.nIdctKernel = ik; }
+void jsimg_config_scan_err_max(jsimg* h, unsigned n) { h->cfg.nErrMaxDecodeScan = n; }
+void jsimg_ScanErrorsDisable(jsimg* h) { h->dec->ScanErrorsDisable(); }
+void jsimg_ScanErrorsEnable(jsimg* h)  { h->dec->ScanErrorsEnable(); }
 void jsimg_config_histo(jsimg* h, int he, int sc, int dy) { h->cfg.bHistoEn = he != 0; h->cfg.bStatClipEn = sc != 0; h->cfg.bDumpHistoY = dy != 0; }
 void jsimg_SetPreviewMode(jsimg* h, unsigned m) { h->dec->SetPreviewMode(m); }
 unsigned jsimg_GetPreviewMode(jsimg* h) { return h->dec->GetPreviewMode(); }

@@ -12,6 +12,7 @@
 #include <cstdarg>
 #include <string>
 #include <vector>
+#include <memory>
 #include <array>
 #include <algorithm>
 #include <dlfcn.h>
@@ -110,6 +111,9 @@ struct jsgpu_ctx {
     DevBuf d_dt_scratch;                     // [16] counters (JsDetailOut::hdr), [JSGPU_HISTO_WORDS] the walk's code-length histogram, then the
                                              // parallel path's per-MCU event counts / offsets and last top-up points
     bool dt_parallel = false; JsDetailRange dt_range = {0, 0, 0, 0, 0}; JsDetailOut dt_out = {};
+    uint32_t scan_warn_start = 0; bool scan_errors_disable = false;      // jsgpu_set_scan_error_state
+    JsErrCfg ex_cfg = {20, 0, 0};            // the error report's settings of the last decode (an events-only walk repeats them)
+    DevBuf d_ex_all;                         // jsgpu_batch_error_events: the walk's result and histogram scratch, then every event
     JsSearch* search = nullptr;              // jsgpu_search_bytes: own streams, staging and device buffers (not the batch pools)
 };
 
@@ -212,6 +216,7 @@ int jsgpu_init(int device, jsgpu_ctx** out)
     for (auto& ev : ctx->tev) cudaEventCreate(&ev);
     memset(&ctx->opt, 0, sizeof ctx->opt);
     ctx->opt.decode_ac = 1; ctx->opt.want_histo = 1; ctx->opt.want_mcu_map = 1; ctx->opt.device_markers = 1;
+    ctx->opt.scan_err_max = 20;                          // CSnoopConfig::nErrMaxDecodeScan's default (SnoopConfig.cpp:89)
     memset(&ctx->batch, 0, sizeof ctx->batch);
     *out = ctx;
     return JSGPU_OK;
@@ -312,6 +317,12 @@ int jsgpu_set_options(jsgpu_ctx* ctx, const jsgpu_options* opt)
     if (!ctx || !opt) return JSGPU_EINVAL;
     if (opt->idct_mode < 0 || opt->idct_mode > 1) return fail(ctx, JSGPU_EINVAL, "idct_mode must be 0 (integer) or 1 (float)");
     ctx->opt = *opt;
+    return JSGPU_OK;
+}
+int jsgpu_set_scan_error_state(jsgpu_ctx* ctx, uint32_t warn_start, int disable)
+{
+    if (!ctx) return JSGPU_EINVAL;
+    ctx->scan_warn_start = warn_start; ctx->scan_errors_disable = disable != 0;
     return JSGPU_OK;
 }
 int jsgpu_get_options(jsgpu_ctx* ctx, jsgpu_options* opt) { if (!ctx || !opt) return JSGPU_EINVAL; *opt = ctx->opt; return JSGPU_OK; }
@@ -628,7 +639,7 @@ int jsgpu_batch_upload(jsgpu_ctx* ctx, const uint8_t* host, uint64_t bytes)
 // run now (a second sync reads the totals, so the arrays are sized exactly), the emit pass after the MCU file map.  Otherwise
 // the serial walk fills arrays sized for the most it can report: 1 + 66 events per block (a separator per MCU; per block a
 // heading, at most 64 symbols, a matrix) and one matrix per block, for the printed MCUs.
-static int detail_prepare(jsgpu_ctx* ctx, int err_max, int* launches)
+static int detail_prepare(jsgpu_ctx* ctx, const JsErrCfg& cfg, int* launches)
 {
     static const bool force_walk = [] { const char* e = getenv("JSGPU_DETAIL_WALK"); return e && atoi(e) == 1; }();
     const DevBatch& b = ctx->batch;
@@ -652,7 +663,7 @@ static int detail_prepare(jsgpu_ctx* ctx, int err_max, int* launches)
     CK(cudaMemsetAsync(hdr, 0, 16 * 4, s));
     uint64_t nev, nmat;
     if (status == 0) {
-        *launches += js_launch_detail_count(b, r, hdr + 16 + JSGPU_HISTO_WORDS, hdr, err_max, s);
+        *launches += js_launch_detail_count(b, r, hdr + 16 + JSGPU_HISTO_WORDS, hdr, cfg, s);
         uint32_t tot[2];
         CK(cudaMemcpyAsync(tot, hdr, sizeof tot, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
@@ -724,18 +735,18 @@ int jsgpu_batch_decode(jsgpu_ctx* ctx)
             launches += js_launch_huffman_lane_vseg(bh, ctx->sm_count, s);
         }
         // the detailed decode of a healthy image: count pass and scan here, events after the MCU file map (below)
-        const int err_max = ctx->opt.scan_err_max > 0 ? ctx->opt.scan_err_max : 20;
+        ctx->ex_cfg = JsErrCfg{ctx->opt.scan_err_max, ctx->scan_warn_start, ctx->scan_errors_disable ? 1u : 0u};
         ctx->dt_done = ctx->dt_parallel = false;
         jsgpu_detail dtl = ctx->dtl;
         if (dtl.enable && dtl.image < b.nimg) {
-            int rc = detail_prepare(ctx, err_max, &launches);
+            int rc = detail_prepare(ctx, ctx->ex_cfg, &launches);
             if (rc != JSGPU_OK) return rc;
             ctx->dt_done = true;
             if (ctx->dt_parallel) dtl.enable = 0;
         } else dtl.enable = 0;
         // damaged images (status word != 0) are decoded again with the reference's semantics (and the detail image, when it takes
         // the serial walk); returns at once for the others
-        launches += js_launch_exact(b, err_max, dtl, ctx->dt_out, ctx->dt_done ? (uint32_t*)ctx->d_dt_scratch.p + 16 : nullptr, s);
+        launches += js_launch_exact(b, ctx->ex_cfg, dtl, ctx->dt_out, ctx->dt_done ? (uint32_t*)ctx->d_dt_scratch.p + 16 : nullptr, s);
     }
     // The MCU file map depends on the Huffman stage only: its kernels run on a second stream while the IDCT kernel has the device
     // (they are short and latency-bound); the scalar statistics below wait for both.
@@ -929,6 +940,30 @@ int jsgpu_batch_errors(jsgpu_ctx* ctx, uint32_t image, jsgpu_scan_errors* out)
     return JSGPU_OK;
 }
 
+int jsgpu_batch_error_events(jsgpu_ctx* ctx, uint32_t image, uint32_t first, uint32_t n, jsgpu_scan_event* out)
+{
+    if (!ctx || (!out && n)) return JSGPU_EINVAL;
+    std::unique_ptr<jsgpu_scan_errors> e(new jsgpu_scan_errors);
+    int rc = jsgpu_batch_errors(ctx, image, e.get());
+    if (rc != JSGPU_OK) return rc;
+    const uint32_t nev = e->nevents;
+    if ((uint64_t)first + n > nev) return fail(ctx, JSGPU_EINVAL, "events %u..%llu asked, image %u has %u", first, (unsigned long long)first + n, image, nev);
+    if ((uint64_t)first + n <= JSGPU_MAX_EVENTS) { memcpy(out, e->ev + first, (size_t)n * sizeof *out); return JSGPU_OK; }
+    // past the first JSGPU_MAX_EVENTS: walk the image again for its events alone, into a buffer sized for all of them
+    const size_t hdr = sizeof(JsExResult) + JSGPU_HISTO_WORDS * 4;
+    CK(ctx->d_ex_all.reserve(hdr + (size_t)nev * sizeof(JsExEvent)));
+    uint8_t* base = (uint8_t*)ctx->d_ex_all.p;
+    JsExEvent* ev = (JsExEvent*)(base + hdr);
+    js_launch_exact_events(ctx->batch, image, ctx->ex_cfg, (JsExResult*)base, (uint32_t*)(base + sizeof(JsExResult)), ev, nev, ctx->stream);
+    CK(cudaGetLastError());
+    uint32_t again = 0;
+    CK(cudaMemcpyAsync(&again, &((JsExResult*)base)->nevents, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(out, ev + first, (size_t)n * sizeof *out, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (again != nev) return fail(ctx, JSGPU_ECUDA, "the events-only walk of image %u found %u events, the decode %u", image, again, nev);
+    return JSGPU_OK;
+}
+
 int jsgpu_batch_checksums(jsgpu_ctx* ctx, uint64_t* ck, uint32_t n)
 {
     if (!ctx || !ck) return JSGPU_EINVAL;
@@ -1037,6 +1072,7 @@ int jsgpu_decode_batch_host(jsgpu_ctx* ctx, const jsgpu_image_desc* imgs, uint32
         // (re)configure the chunk context like this one
         jsgpu_options o = ctx->opt;
         r = jsgpu_set_options(k, &o); if (r) return fail(ctx, r, "%s", k->err.c_str());
+        k->scan_warn_start = ctx->scan_warn_start; k->scan_errors_disable = ctx->scan_errors_disable;
         k->pv = ctx->pv;
         if (!k->have_idct || k->h_li != ctx->h_li) { r = jsgpu_set_idct_tables(k, ctx->h_li.data(), ctx->h_lf.data()); if (r) return fail(ctx, r, "%s", k->err.c_str()); }
         if (k->h_sets.size() != ctx->h_sets.size() || memcmp(k->h_sets.data(), ctx->h_sets.data(), sizeof(jsgpu_tables) * ctx->h_sets.size()) != 0) {

@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(DT_THREADS) k_detail_count(DevBatch b, JsDetai
     lastp[j] = lp;
 }
 
-__global__ void __launch_bounds__(1024) k_detail_scan(DevBatch b, JsDetailRange r, uint32_t* cnt, const uint32_t* lastp, uint32_t* hdr, int err_max)
+__global__ void __launch_bounds__(1024) k_detail_scan(DevBatch b, JsDetailRange r, uint32_t* cnt, const uint32_t* lastp, uint32_t* hdr, JsErrCfg cfg)
 {
     __shared__ uint32_t s_warp[32];
     __shared__ uint32_t s_carry;
@@ -164,8 +164,9 @@ __global__ void __launch_bounds__(1024) k_detail_scan(DevBatch b, JsDetailRange 
     if (tid != 0) return;
     const DevImage& im = b.img[r.image];
     hdr[0] = s_carry; hdr[1] = r.nprint * im.bpm;
-    // the end-of-scan marker note (BuffAddByte, ImgDecode.cpp:1527-1543) when the walk's last top-up reaches it, plus the cap line
-    // when the cap is 1 (:1100-1110); the fields the walk sets for a healthy image, the others as they were
+    // the end-of-scan marker note (BuffAddByte, ImgDecode.cpp:1527-1543) when the walk's last top-up reaches it and the cap still
+    // allows a line, plus the cap line when this one reaches it (:1100-1110); the fields the walk sets for a healthy image, the
+    // others as they were
     uint32_t marker;
     const long long T = dt_marker_threshold(b, im, r.image, marker);
     bool met;
@@ -173,13 +174,15 @@ __global__ void __launch_bounds__(1024) k_detail_scan(DevBatch b, JsDetailRange 
     else met = im.nseg == 1 && 0 >= T;                           // nothing decoded: the first top-up only
     JsExResult* res = b.ex_res + r.image;
     res->nerr_lines = 0; res->nevents = 0; res->scan_bad = 0; res->restart_read = 0; res->done = 0;
-    if (met && err_max > 0) {
+    res->warn_num = cfg.warn_start;
+    if (met && cfg.warn_start < cfg.err_max) {
         JsExEvent& e = res->ev[0];
         e.code = JS_EX_MARKER_NOTE; e.a = marker; e.b = im.file_pos + b.scan_end[r.image]; e.c = e.d = e.e = 0; e.pad0 = e.pad1 = 0;
         res->nevents = 1; res->nerr_lines = (marker != 0xD9) ? 1u : 0u;
-        if (err_max <= 1) {
+        res->warn_num = cfg.warn_start + 1;
+        if (res->warn_num >= cfg.err_max) {
             JsExEvent& c = res->ev[1];
-            c.code = JS_EX_CAP; c.a = (uint32_t)err_max; c.b = c.c = c.d = c.e = 0; c.pad0 = c.pad1 = 0;
+            c.code = JS_EX_CAP; c.a = cfg.err_max; c.b = c.c = c.d = c.e = 0; c.pad0 = c.pad1 = 0;
             res->nevents = 2; res->nerr_lines++;
         }
     }
@@ -200,12 +203,12 @@ __global__ void __launch_bounds__(DT_THREADS) k_detail_emit(DevBatch b, JsDetail
     dt_mcu<true, false>(b, im, m, T, b.ex_res[r.image].nevents, prev_met, out.ev + off[jj], out.mat, j * im.bpm, lp);
 }
 
-int js_launch_detail_count(const DevBatch& b, const JsDetailRange& r, uint32_t* scratch, uint32_t* hdr, int err_max, cudaStream_t s)
+int js_launch_detail_count(const DevBatch& b, const JsDetailRange& r, uint32_t* scratch, uint32_t* hdr, const JsErrCfg& cfg, cudaStream_t s)
 {
     uint32_t* cnt = scratch; uint32_t* lastp = scratch + r.n;
     int n = 0;
     if (r.n) { k_detail_count<<<(r.n + DT_THREADS - 1) / DT_THREADS, DT_THREADS, 0, s>>>(b, r, cnt, lastp, b.decode_ac ? 0 : 1); n++; }
-    k_detail_scan<<<1, 1024, 0, s>>>(b, r, cnt, lastp, hdr, err_max);
+    k_detail_scan<<<1, 1024, 0, s>>>(b, r, cnt, lastp, hdr, cfg);
     return n + 1;
 }
 

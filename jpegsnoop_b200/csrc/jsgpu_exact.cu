@@ -26,9 +26,10 @@ struct Ex {
     uint32_t pos[4], err[4], latch_err, num, align;
     bool scan_end, scan_bad, cur_err, restart_flag;
     uint32_t restart_read, restart_last, restart_expect, mcus_left, rst_interval, warn_bad_num, err_max;
-    uint32_t precision; bool decode_ac;
+    uint32_t precision; bool decode_ac, errs_off;     // errs_off: m_bScanErrorsDisable
     short css[3][16];                            // m_anDcLumCss / m_anDcChrCbCss / m_anDcChrCrCss: DC sum of block (v,h) of the current MCU
     JsExResult* res;
+    JsExEvent* ev; uint32_t ev_cap;              // where events 0 .. ev_cap-1 go (res->ev and its 256 normally; every event of an events-only walk)
     uint32_t* histo;                             // [2][4][17] of this image
     const DevTableSet* ts;
     short dct[64];
@@ -51,7 +52,7 @@ __device__ __forceinline__ void ex_event(Ex& x, uint32_t code, uint32_t lines, u
 {
     JsExResult* r = x.res;
     r->nerr_lines += lines;
-    if (r->nevents < JS_EX_MAX_EVENTS) { JsExEvent& ev = r->ev[r->nevents]; ev.code = code; ev.a = a; ev.b = b; ev.c = c; ev.d = d; ev.e = e; ev.pad0 = ev.pad1 = 0; }
+    if (r->nevents < x.ev_cap) { JsExEvent& ev = x.ev[r->nevents]; ev.code = code; ev.a = a; ev.b = b; ev.c = c; ev.d = d; ev.e = e; ev.pad0 = ev.pad1 = 0; }
     r->nevents++;
 }
 // the "first nErrMaxDecodeScan instances" pattern (ImgDecode.cpp:1100-1110 and its copies)
@@ -96,7 +97,7 @@ __device__ __noinline__ void ex_buff_add_byte(Ex& x)
         marker = b1;
         if (marker >= 0xD0 && marker <= 0xD7) {
             x.restart_read++; x.restart_last = marker - 0xD0;
-            if (x.restart_last != x.restart_expect) ex_event(x, JS_EX_RST_MISMATCH, 1, x.restart_expect, x.restart_last, x.file_pos + x.ptr);
+            if (x.restart_last != x.restart_expect && !x.errs_off) ex_event(x, JS_EX_RST_MISMATCH, 1, x.restart_expect, x.restart_last, x.file_pos + x.ptr);
             x.restart_expect = (x.restart_last + 1) % 8;
             x.restart_flag = true;
             return;
@@ -245,20 +246,23 @@ __device__ __noinline__ bool ex_decode_scan_comp(Ex& x, uint32_t tdc, uint32_t t
 // The same walk serves the "Detailed Decode" of chosen MCUs (m_bDetailVlc, SetDetailVlc :4898) of a damaged image, and of a healthy
 // one when the parallel form (jsgpu_detail.cu) is not taken (JSGPU_DETAIL_WALK=1, no MCU file map) — then without touching any output (the fast path has produced them) except the
 // coefficient rows of the printed MCUs in DC-only mode, which the reference decodes in full — and ends after the last MCU of the range.
-__global__ void __launch_bounds__(32) k_huff_exact(DevBatch b, int err_max, jsgpu_detail dtl, JsDetailOut dump, uint32_t* scratch_histo)
+// With ev_all set it is the events-only walk of image ii (jsgpu_batch_error_events): the whole scan, every event into ev_all, the
+// counts into res, nothing else written.  The walk depends only on the resident scan, the tables and cfg, so it repeats the events.
+__device__ __forceinline__ void ex_walk(const DevBatch& b, uint32_t ii, const JsErrCfg& cfg, const jsgpu_detail& dtl, const JsDetailOut& dump,
+                                        uint32_t* scratch_histo, JsExResult* res, JsExEvent* ev_all, uint32_t ev_cap)
 {
-    const uint32_t ii = blockIdx.x;
-    if (threadIdx.x != 0) return;
-    const bool wr = b.ex_flag[ii] != 0;                          // damaged: this walk produces the outputs
-    const bool detail = dtl.enable && dtl.image == ii && b.img[ii].valid;
-    if (!wr && !detail) return;
+    const bool evonly = ev_all != nullptr;
+    const bool wr = !evonly && b.ex_flag[ii] != 0;              // damaged: this walk produces the outputs
+    const bool detail = !evonly && dtl.enable && dtl.image == ii && b.img[ii].valid;
+    if (!wr && !detail && !evonly) return;
     const DevImage& im = b.img[ii];
     Ex x;
     x.data = b.bits + im.scan_off; x.n = (uint32_t)im.scan_len; x.file_pos = im.file_pos;
     x.ts = b.tables + im.table_set;
-    x.res = b.ex_res + ii; x.histo = wr ? b.histo + (size_t)ii * JSGPU_HISTO_WORDS : scratch_histo;
+    x.res = res; x.histo = wr ? b.histo + (size_t)ii * JSGPU_HISTO_WORDS : scratch_histo;
+    x.ev = evonly ? ev_all : res->ev; x.ev_cap = evonly ? ev_cap : JS_EX_MAX_EVENTS;
     x.res->nerr_lines = 0; x.res->nevents = 0; x.res->scan_bad = 0; x.res->restart_read = 0; x.res->done = 0;
-    x.err_max = (uint32_t)err_max; x.warn_bad_num = 0;
+    x.err_max = cfg.err_max; x.warn_bad_num = cfg.warn_start; x.errs_off = cfg.disable != 0;
     x.precision = im.precision; x.decode_ac = b.decode_ac != 0;
     x.rst_interval = im.restart_en ? im.ri : 0;                 // m_nRestartInterval (0 when DRI is off: never looked at then)
     x.restart_read = 0; x.restart_last = 0; x.restart_expect = 0; x.bits_used = 0;
@@ -276,7 +280,7 @@ __global__ void __launch_bounds__(32) k_huff_exact(DevBatch b, int err_max, jsgp
         bool stop = false;
         for (uint32_t mx = 0; mx < im.mcu_xmax && !stop; mx++) {
             const uint32_t mcu = my * im.mcu_xmax + mx;
-            if (!wr && (unsigned long long)mcu >= (unsigned long long)dt_base + dtl.len) { all_done = true; break; }     // nothing left to print
+            if (detail && !wr && (unsigned long long)mcu >= (unsigned long long)dt_base + dtl.len) { all_done = true; break; }     // nothing left to print
             if (im.restart_en && x.mcus_left == 0 && !x.restart_flag) ex_event(x, JS_EX_RST_MISSING, 1, x.pos[0], x.align);     // :3180-3200
             if (wr) b.mcu_map[im.mcu_off + mcu] = (x.pos[0] << 4) + x.align;                                                       // :3229
             const bool print = detail && mcu >= dt_base && (unsigned long long)mcu < (unsigned long long)dt_base + dtl.len;        // :3235-3241
@@ -312,11 +316,22 @@ __global__ void __launch_bounds__(32) k_huff_exact(DevBatch b, int err_max, jsgp
             if (x.scan_end && x.scan_bad) stop = true;           // :3621-3625
         }
     }
+    x.res->warn_num = x.warn_bad_num;
     if (!wr) return;
     x.res->scan_bad = x.scan_bad ? 1u : 0u; x.res->restart_read = x.restart_read; x.res->done = 1;
     x.res->end_pos = x.pos[0]; x.res->end_align = x.align;
     b.stats[(size_t)ii * JSGPU_STAT_WORDS + 11] = (int32_t)x.restart_read;     // m_nRestartRead
     b.stats[(size_t)ii * JSGPU_STAT_WORDS + 12] = (int32_t)x.pos[0]; b.stats[(size_t)ii * JSGPU_STAT_WORDS + 13] = (int32_t)x.align;
+}
+
+__global__ void __launch_bounds__(32) k_huff_exact(DevBatch b, JsErrCfg cfg, jsgpu_detail dtl, JsDetailOut dump, uint32_t* scratch_histo)
+{
+    if (threadIdx.x == 0) ex_walk(b, blockIdx.x, cfg, dtl, dump, scratch_histo, b.ex_res + blockIdx.x, nullptr, 0);
+}
+__global__ void __launch_bounds__(32) k_huff_exact_events(DevBatch b, uint32_t image, JsErrCfg cfg, JsExResult* res, uint32_t* scratch_histo, JsExEvent* ev, uint32_t ev_cap)
+{
+    const jsgpu_detail none = {0, 0, 0, 0, 0};
+    if (threadIdx.x == 0) ex_walk(b, image, cfg, none, JsDetailOut{}, scratch_histo, res, ev, ev_cap);
 }
 
 // Before the re-decode: which images need it, and their intermediates back to the state the reference starts from
@@ -339,10 +354,16 @@ __global__ void __launch_bounds__(256) k_exact_prepare(DevBatch b)
     for (uint32_t i = threadIdx.x; i < JSGPU_HISTO_WORDS; i += blockDim.x) b.histo[(size_t)ii * JSGPU_HISTO_WORDS + i] = 0;
 }
 
-int js_launch_exact(const DevBatch& b, int err_max, const jsgpu_detail& dtl, const JsDetailOut& dump, uint32_t* scratch_histo, cudaStream_t s)
+int js_launch_exact(const DevBatch& b, const JsErrCfg& cfg, const jsgpu_detail& dtl, const JsDetailOut& dump, uint32_t* scratch_histo, cudaStream_t s)
 {
     if (b.nimg == 0) return 0;
     k_exact_prepare<<<b.nimg, 256, 0, s>>>(b);
-    k_huff_exact<<<b.nimg, 32, 0, s>>>(b, err_max, dtl, dump, scratch_histo);
+    k_huff_exact<<<b.nimg, 32, 0, s>>>(b, cfg, dtl, dump, scratch_histo);
     return 2;
+}
+
+int js_launch_exact_events(const DevBatch& b, uint32_t image, const JsErrCfg& cfg, JsExResult* res, uint32_t* scratch_histo, JsExEvent* ev, uint32_t ev_cap, cudaStream_t s)
+{
+    k_huff_exact_events<<<1, 32, 0, s>>>(b, image, cfg, res, scratch_histo, ev, ev_cap);
+    return 1;
 }

@@ -187,8 +187,12 @@ struct JsDetailOut {
 };
 // ... and, for the parallel path (jsgpu_detail.cu), which MCUs: first .. first+n-1 are decoded, base .. base+nprint-1 printed
 struct JsDetailRange { uint32_t image, base, first, n, nprint; };
-int js_launch_exact(const DevBatch& b, int err_max, const jsgpu_detail& dtl, const JsDetailOut& dump, uint32_t* scratch_histo, cudaStream_t s);       // damaged images, again, with the reference's semantics (jsgpu_exact.cu)
-int js_launch_detail_count(const DevBatch& b, const JsDetailRange& r, uint32_t* scratch, uint32_t* hdr, int err_max, cudaStream_t s);   // count pass + scan (+ DC-only rows)
+// the error report's state at the start of a scan: m_nScanErrMax, m_nWarnBadScanNum, m_bScanErrorsDisable
+struct JsErrCfg { uint32_t err_max, warn_start, disable; };
+int js_launch_exact(const DevBatch& b, const JsErrCfg& cfg, const jsgpu_detail& dtl, const JsDetailOut& dump, uint32_t* scratch_histo, cudaStream_t s);       // damaged images, again, with the reference's semantics (jsgpu_exact.cu)
+// the same walk of one image for its events alone (no output is written): events 0 .. ev_cap-1 go to ev, the counts to *res
+int js_launch_exact_events(const DevBatch& b, uint32_t image, const JsErrCfg& cfg, JsExResult* res, uint32_t* scratch_histo, JsExEvent* ev, uint32_t ev_cap, cudaStream_t s);
+int js_launch_detail_count(const DevBatch& b, const JsDetailRange& r, uint32_t* scratch, uint32_t* hdr, const JsErrCfg& cfg, cudaStream_t s);   // count pass + scan (+ DC-only rows)
 int js_launch_detail_emit(const DevBatch& b, const JsDetailRange& r, const uint32_t* scratch, const JsDetailOut& out, cudaStream_t s);  // events + matrices (after the MCU file map)
 int js_launch_export(const DevBatch& b, uint32_t image, int mode, uint8_t* out, uint64_t npx, int sm_count, cudaStream_t s);   // Export-to-TIFF sample array
 int js_launch_finalize_maps(const DevBatch& b, cudaStream_t s);     // MCU file map (independent of the IDCT)

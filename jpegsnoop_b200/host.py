@@ -81,6 +81,13 @@ class CimgDecode:
     def config_histo(self, histo_en=False, statclip_en=False, dump_histo_y=False):
         self.L.jsimg_config_histo(self.h, int(histo_en), int(statclip_en), int(dump_histo_y))
 
+    def config_scan_err_max(self, n):
+        """CSnoopConfig::nErrMaxDecodeScan: how many of each capped scan error line a decode reports (0: none; default 20)."""
+        self.L.jsimg_config_scan_err_max(self.h, n)
+
+    def ScanErrorsDisable(self): self.L.jsimg_ScanErrorsDisable(self.h)
+    def ScanErrorsEnable(self): self.L.jsimg_ScanErrorsEnable(self.h)
+
     def SetPreviewMode(self, mode): self.L.jsimg_SetPreviewMode(self.h, mode)
     def GetPreviewMode(self): return int(self.L.jsimg_GetPreviewMode(self.h))
     def SetPreviewYccOffset(self, mx, my, y, cb, cr): self.L.jsimg_SetPreviewYccOffset(self.h, mx, my, y, cb, cr)
@@ -307,7 +314,7 @@ class BatchDecoder:
         self._ck(self.L.jsgpu_set_idct_tables(self.ctx, li.ctypes.data, lf.ctypes.data))
         self.opt = B.jsgpu_options(idct_mode=0 if idct_fixedpt else 1, decode_ac=int(decode_ac), huff_kernel=huff_kernel,
                                    idct_kernel=idct_kernel, want_histo=int(want_histo), want_mcu_map=int(want_mcu_map),
-                                   scan_err_max=0)
+                                   scan_err_max=20)
         self._ck(self.L.jsgpu_set_options(self.ctx, C.byref(self.opt)))
         self.n = 0; self.layout = None; self.descs = None; self.bitstream = None; self.nsof_pixels = 0
 
@@ -480,6 +487,13 @@ class BatchDecoder:
     def scan_errors(self, i):
         """jsgpu_scan_errors of image i (only for images whose status carries JSGPU_ST_EXACT = 0x40000000)."""
         e = B.jsgpu_scan_errors(); self._ck(self.L.jsgpu_batch_errors(self.ctx, i, C.byref(e))); return e
+
+    def scan_error_events(self, i):
+        """Every error event of image i (jsgpu_batch_error_events), not only the first 256: uint32 [nevents, 8] with the
+        columns of jsgpu_scan_event (code, a, b, c, d, e, pad0, pad1)."""
+        n = int(self.scan_errors(i).nevents)
+        ev = np.zeros((n, 8), np.uint32)
+        self._ck(self.L.jsgpu_batch_error_events(self.ctx, i, 0, n, ev.ctypes.data)); return ev
 
     def checksums(self):
         """uint64 [n][12]: device-side checksums of every output buffer of every image (include/jsgpu.h)."""

@@ -162,7 +162,12 @@ class Oracle:
         r = self._f("decode_jpeg")(self.ctx, buf.ctypes.data, buf.size, 1 if quiet else 0)
         if r < 0:
             raise ValueError(f"marker walk failed ({r})")
-        d = Decoded(); d.scan_start = r
+        d = self.collect(); d.scan_start = r
+        return d
+
+    def collect(self):
+        """Decoded copy of everything the last DecodeScanImg left behind (scan_start not set)."""
+        d = Decoded()
         g = np.zeros(8, np.uint32); self._f("geometry")(self.ctx, g.ctypes.data); d.geom = g
         Wp, Hp = int(g[6]), int(g[7])
         nblk = int(g[4]) * int(g[5]); nmcu = int(g[2]) * int(g[3])
