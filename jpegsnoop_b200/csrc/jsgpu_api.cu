@@ -19,23 +19,6 @@
 
 #define JSGPU_VERSION 100
 
-struct DevBuf {
-    void* p = nullptr; size_t cap = 0;
-    DevBuf() = default;
-    DevBuf(const DevBuf&) = delete;
-    DevBuf& operator=(const DevBuf&) = delete;
-    ~DevBuf() { if (p) cudaFree(p); }
-    cudaError_t reserve(size_t n) {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
-        size_t want = n + n / 8 + 256;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-};
-
 // Lays out consecutive arrays in one pool.  Run once with base == nullptr to measure the bytes to reserve, then on the
 // reserved block to bind the pointers; align(a) counts a whole `a` bytes while measuring (the most it can skip).
 struct Carve {

@@ -17,6 +17,29 @@
 #define JS_H100_SMS   132u               // grid-size heuristics of the small helper kernels (the main kernels take the device's SM count)
 #define JS_NSLOT      8                  // (class,Th) pairs: slot = class*4 + Th
 
+// An owning, growable buffer of device memory (DevBuf) or pinned host memory (PinBuf).  reserve(n) keeps it while it holds
+// n bytes; otherwise it is replaced, contents lost, by one of n + n/8 + 256 bytes, so that slowly growing sizes rarely reallocate.
+template <cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
+struct OwnedBuf {
+    void* p = nullptr; size_t cap = 0;
+    OwnedBuf() = default;
+    OwnedBuf(const OwnedBuf&) = delete;
+    OwnedBuf& operator=(const OwnedBuf&) = delete;
+    ~OwnedBuf() { if (p) Free(p); }
+    cudaError_t reserve(size_t n) {
+        if (n <= cap) return cudaSuccess;
+        if (p) Free(p);
+        p = nullptr; cap = 0;
+        size_t want = n + n / 8 + 256;
+        cudaError_t e = Alloc(&p, want);
+        if (e == cudaSuccess) cap = want;
+        return e;
+    }
+    template <class T> T* as() const { return (T*)p; }
+};
+using DevBuf = OwnedBuf<cudaMalloc, cudaFree>;
+using PinBuf = OwnedBuf<cudaMallocHost, cudaFreeHost>;
+
 // serial reference-semantics path (jsgpu_exact.cu): per-image result = the public jsgpu_scan_errors
 typedef jsgpu_scan_errors JsExResult; typedef jsgpu_scan_event JsExEvent;
 #define JS_EX_MAX_EVENTS JSGPU_MAX_EVENTS

@@ -25,12 +25,78 @@
 #include <cstring>
 #include <vector>
 #include <algorithm>
+#include <memory>
 
-#define SR_TILE     4096                 // positions per tile
-#define SR_THREADS  256                  // 16 consecutive positions per thread
+#define SR_THREADS  256                  // threads per CTA of the tile kernels
+#define SR_TILE     (SR_THREADS * 16)    // positions per tile: 16 consecutive positions per thread
 #define SR_HALO     272                  // bytes staged past the tile: maxlen - 1 (<= 255) and the 8-byte window, rounded to 16
 #define SR_HBITS    16                   // prefix hash width
 #define SR_WORDS    (SR_TILE / 32)       // match-bitmap words per pattern and tile
+
+// ---- scans: every kernel's, over any T of 32-bit words and any associative op (op(a, b): a, then b) with identity id ----
+template <typename T, typename F>
+__device__ __forceinline__ T sr_shfl(T x, F f)             // f (a shuffle) applied to each 32-bit word of x
+{
+    static_assert(sizeof(T) % 4 == 0, "shuffled as 32-bit words");
+    uint32_t w[sizeof(T) / 4];
+    memcpy(w, &x, sizeof(T));
+#pragma unroll
+    for (int i = 0; i < (int)(sizeof(T) / 4); i++) w[i] = f(w[i]);
+    memcpy(&x, w, sizeof(T));
+    return x;
+}
+
+// Over lanes 0 .. W-1 (W a power of two; the whole warp calls): returns the exclusive prefix of v, id in lane 0, and sets
+// `inc` to the inclusive one.
+template <int W = 32, typename T, typename Op>
+__device__ __forceinline__ T warp_scan(T v, T id, Op op, T& inc)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    inc = v;
+#pragma unroll
+    for (int d = 1; d < W; d <<= 1) {
+        const T o = sr_shfl(inc, [d](uint32_t x) { return __shfl_up_sync(0xffffffffu, x, d); });
+        if (lane >= (uint32_t)d) inc = op(o, inc);
+    }
+    const T ex = sr_shfl(inc, [](uint32_t x) { return __shfl_up_sync(0xffffffffu, x, 1); });
+    return lane ? ex : id;
+}
+__device__ __forceinline__ uint32_t sr_add(uint32_t a, uint32_t b) { return a + b; }
+
+// Over a CTA of NT threads, after `carry` (the same in every thread): returns carry op (the values of the threads before
+// this one) and advances `carry` by the whole CTA's.  s_w: NT / 32 + 1 elements of shared memory, free again at the next
+// call.  Up to 8 warps, every thread combines the warp totals itself, which takes no barrier after that of the totals.
+// With more, 32 serial steps in every thread would cost more than a barrier: warp 0 scans the totals for all.
+template <int NT, typename T, typename Op>
+__device__ __forceinline__ T block_scan(T v, T id, Op op, T& carry, T* s_w)
+{
+    constexpr uint32_t NW = NT / 32;
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    T inc, before = carry;
+    const T ex = warp_scan(v, id, op, inc);
+    __syncthreads();                                          // the previous call is done with s_w
+    if (lane == 31) s_w[warp] = inc;
+    __syncthreads();
+    if constexpr (NW <= 8) {
+#pragma unroll
+        for (uint32_t k = 0; k < NW; k++) {
+            const T w = s_w[k];
+            if (k < warp) before = op(before, w);
+            carry = op(carry, w);
+        }
+    } else {
+        if (warp == 0) {                                      // s_w[w] becomes carry op the warps before w, s_w[NW] the new carry
+            const T wex = warp_scan<NW>(lane < NW ? s_w[lane] : id, id, op, inc);
+            __syncwarp();
+            if (lane < NW) s_w[lane] = op(carry, wex);
+            if (lane == NW - 1) s_w[NW] = op(carry, inc);
+        }
+        __syncthreads();
+        before = s_w[warp];
+        carry = s_w[NW];
+    }
+    return op(before, ex);
+}
 
 struct SrParams {
     uint32_t npat, maxlen;
@@ -149,14 +215,8 @@ k_search_tiles(const uint8_t* __restrict__ chunk, uint64_t chunk_pos, uint64_t v
         // one warp per pattern: lane l owns positions 128 l .. 128 l + 127 as two 64-bit words
         for (uint32_t k = warp; k < npat; k += SR_THREADS / 32) {
             const uint64_t b0 = ((const uint64_t*)s_match[k])[2 * lane], b1 = ((const uint64_t*)s_match[k])[2 * lane + 1];
-            uint32_t f = sr_then(sr_word_map(b0), sr_word_map(b1)), inc = f;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const uint32_t o = __shfl_up_sync(0xffffffffu, inc, d);
-                if (lane >= (uint32_t)d) inc = sr_then(o, inc);
-            }
-            uint32_t pre = __shfl_up_sync(0xffffffffu, inc, 1);
-            if (lane == 0) pre = 2u;
+            uint32_t inc;
+            const uint32_t pre = warp_scan(sr_then(sr_word_map(b0), sr_word_map(b1)), 2u, sr_then, inc);
             if (!EMIT) {
                 const uint32_t tot = __shfl_sync(0xffffffffu, inc, 31);
                 uint64_t r0, r1;
@@ -169,14 +229,8 @@ k_search_tiles(const uint8_t* __restrict__ chunk, uint64_t chunk_pos, uint64_t v
                 const uint32_t o = s_tin[k];
                 uint64_t r0, r1;
                 sr_lane_bits(b0, b1, pre, o & 1u, r0, r1);
-                const uint32_t n = (uint32_t)(__popcll(r0) + __popcll(r1));
-                uint32_t ex = n;
-#pragma unroll
-                for (int d = 1; d < 32; d <<= 1) {
-                    const uint32_t v = __shfl_up_sync(0xffffffffu, ex, d);
-                    if (lane >= (uint32_t)d) ex += v;
-                }
-                uint32_t j = (o >> 1) + ex - n;                  // chunk-local output index of this lane's first position
+                uint32_t n_inc;                                  // j: chunk-local output index of this lane's first position
+                uint32_t j = (o >> 1) + warp_scan((uint32_t)(__popcll(r0) + __popcll(r1)), 0u, sr_add, n_inc);
                 const uint32_t fp0 = (uint32_t)(chunk_pos + tb) + 128 * lane;
                 for (int h = 0; h < 2; h++) {
                     uint64_t r = h ? r1 : r0;
@@ -207,86 +261,58 @@ __global__ void __launch_bounds__(1024)
 k_search_scan(const uint32_t* __restrict__ summ, uint32_t ntiles, uint32_t* __restrict__ toff, uint32_t* __restrict__ chunk_res,
               uint32_t chunk, uint32_t npat)
 {
-    __shared__ SrMap s_w[32];
-    __shared__ uint32_t s_r, s_tot;
-    const uint32_t k = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    // chunk_res[c][k] = {count, outgoing flag}
-    if (tid == 0) { s_r = chunk ? chunk_res[2 * ((size_t)(chunk - 1) * npat + k) + 1] : 0u; s_tot = 0; }
-    __syncthreads();
+    __shared__ SrMap s_w[33];
+    const uint32_t k = blockIdx.x, tid = threadIdx.x;
+    const SrMap id = {0u, 1u, 0u, 0u};
+    // chunk_res[c][k] = {count, outgoing flag}; r: the flag the chunk starts with
+    const uint32_t r = chunk ? chunk_res[2 * ((size_t)(chunk - 1) * npat + k) + 1] : 0u;
+    SrMap all = id;                                           // the map of the tiles scanned so far
     for (uint32_t t0 = 0; t0 < ntiles; t0 += 1024) {
         const uint32_t t = t0 + tid;
-        SrMap m = {0u, 1u, 0u, 0u};                            // identity
+        SrMap m = id;
         if (t < ntiles) {
             const uint32_t s = summ[(size_t)k * ntiles + t];
             m.c0 = s & 0xFFFu; m.c1 = (s >> 12) & 0xFFFu; m.o0 = (s >> 24) & 1u; m.o1 = (s >> 25) & 1u;
         }
-        SrMap inc = m;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            SrMap o;
-            o.o0 = __shfl_up_sync(0xffffffffu, inc.o0, d); o.o1 = __shfl_up_sync(0xffffffffu, inc.o1, d);
-            o.c0 = __shfl_up_sync(0xffffffffu, inc.c0, d); o.c1 = __shfl_up_sync(0xffffffffu, inc.c1, d);
-            if (lane >= (uint32_t)d) inc = sr_compose(o, inc);
-        }
-        if (lane == 31) s_w[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-            SrMap v = s_w[lane];
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                SrMap o;
-                o.o0 = __shfl_up_sync(0xffffffffu, v.o0, d); o.o1 = __shfl_up_sync(0xffffffffu, v.o1, d);
-                o.c0 = __shfl_up_sync(0xffffffffu, v.c0, d); o.c1 = __shfl_up_sync(0xffffffffu, v.c1, d);
-                if (lane >= (uint32_t)d) v = sr_compose(o, v);
-            }
-            s_w[lane] = v;                                    // inclusive over warps
-        }
-        __syncthreads();
-        const uint32_t r = s_r, tot = s_tot;
-        SrMap ex = {0u, 1u, 0u, 0u};
-        if (warp) ex = s_w[warp - 1];
-        SrMap in_warp;                                        // exclusive inside the warp
-        in_warp.o0 = __shfl_up_sync(0xffffffffu, inc.o0, 1); in_warp.o1 = __shfl_up_sync(0xffffffffu, inc.o1, 1);
-        in_warp.c0 = __shfl_up_sync(0xffffffffu, inc.c0, 1); in_warp.c1 = __shfl_up_sync(0xffffffffu, inc.c1, 1);
-        if (lane) ex = sr_compose(ex, in_warp);
-        if (t < ntiles) {
-            const uint32_t rin = r ? ex.o1 : ex.o0, off = tot + (r ? ex.c1 : ex.c0);
-            toff[(size_t)k * ntiles + t] = (off << 1) | rin;
-        }
-        __syncthreads();
-        if (tid == 0) { const SrMap all = s_w[31]; s_tot = tot + (r ? all.c1 : all.c0); s_r = r ? all.o1 : all.o0; }
-        __syncthreads();
+        const SrMap ex = block_scan<1024>(m, id, sr_compose, all, s_w);
+        if (t < ntiles) toff[(size_t)k * ntiles + t] = ((r ? ex.c1 : ex.c0) << 1) | (r ? ex.o1 : ex.o0);
     }
-    if (tid == 0) { chunk_res[2 * ((size_t)chunk * npat + k)] = s_tot; chunk_res[2 * ((size_t)chunk * npat + k) + 1] = s_r; }
+    if (tid == 0) {
+        chunk_res[2 * ((size_t)chunk * npat + k)] = r ? all.c1 : all.c0;
+        chunk_res[2 * ((size_t)chunk * npat + k) + 1] = r ? all.o1 : all.o0;
+    }
 }
 
-// ---- host side -------------------------------------------------------------------------------------------------------
+// ---- host side: one chunk pipeline for the three searches --------------------------------------------------------------
+// Two slots, each a pinned staging buffer, a device chunk buffer and a stream: the host stages chunk k + 1 into one slot
+// while the device searches chunk k from the other.  copied[i] follows slot i's last upload; scanned[i] its last scan
+// kernel, through which the scans of consecutive chunks are chained across the two streams.
 struct JsSearch {
     int device = -1;
-    cudaStream_t st[2] = {nullptr, nullptr};
-    cudaEvent_t copied[2] = {nullptr, nullptr}, scanned[2] = {nullptr, nullptr};
-    uint8_t* pin[2] = {nullptr, nullptr}; size_t pin_cap = 0;
-    uint8_t* dbuf[2] = {nullptr, nullptr}; size_t dbuf_cap = 0;
-    uint32_t* dsum[2] = {nullptr, nullptr}; uint32_t* doff[2] = {nullptr, nullptr}; size_t tile_cap = 0;
-    uint8_t* dpat = nullptr; uint32_t* dhash = nullptr;
-    uint32_t* dres = nullptr; size_t res_cap = 0;
-    uint32_t* dout = nullptr; size_t out_cap = 0;
-    uint32_t* dfind = nullptr; uint32_t* hfind = nullptr;   // jsgpu_find_value: one result word per slot, device and pinned host
-    uint32_t* dfa[2] = {nullptr, nullptr}; size_t fa_cap = 0;   // jsgpu_find_all: per-CTA counts and output indices per slot
+    cudaStream_t st[2] = {};
+    cudaEvent_t copied[2] = {}, scanned[2] = {};
+    PinBuf pin[2];
+    DevBuf buf[2];
+    DevBuf sum[2], off[2];                  // jsgpu_search_bytes: tile summaries and output offsets per slot ...
+    DevBuf pat, hash, res;                  // ... the patterns, their prefix hash, and each chunk's counts and outgoing flags
+    DevBuf out;                             // jsgpu_search_bytes (one chunk's) and jsgpu_find_all: the positions
+    DevBuf find; PinBuf hfind;              // jsgpu_find_value: one result word per slot, device and pinned host
+    DevBuf cta[2], total;                   // jsgpu_find_all: per slot the per-CTA counts and output indices; the running count
+    ~JsSearch()
+    {
+        for (int i = 0; i < 2; i++) {
+            if (copied[i]) cudaEventDestroy(copied[i]);
+            if (scanned[i]) cudaEventDestroy(scanned[i]);
+            if (st[i]) cudaStreamDestroy(st[i]);
+        }
+    }
 };
 
 void js_search_free(JsSearch* s)
 {
     if (!s) return;
     cudaSetDevice(s->device);
-    for (int i = 0; i < 2; i++) {
-        if (s->st[i]) cudaStreamSynchronize(s->st[i]);
-        cudaFreeHost(s->pin[i]); cudaFree(s->dbuf[i]); cudaFree(s->dsum[i]); cudaFree(s->doff[i]); cudaFree(s->dfa[i]);
-        if (s->copied[i]) cudaEventDestroy(s->copied[i]);
-        if (s->scanned[i]) cudaEventDestroy(s->scanned[i]);
-        if (s->st[i]) cudaStreamDestroy(s->st[i]);
-    }
-    cudaFree(s->dpat); cudaFree(s->dhash); cudaFree(s->dres); cudaFree(s->dout); cudaFree(s->dfind); cudaFreeHost(s->hfind);
+    for (cudaStream_t t : s->st) cudaStreamSynchronize(t);
     delete s;
 }
 
@@ -298,55 +324,68 @@ static uint64_t sr_chunk_bytes()
     return std::min<uint64_t>(c, 128ull << 20);               // keeps every per-chunk count and output index within 32 bits
 }
 
+// The positions lo .. lo + npos - 1 in chunks of `size` (a multiple of the tile), in search order: upward, or from the top
+// when `down`.  Chunk c's bytes are those of its positions and the `halo` bytes after them, as far as the file's n go.
+struct SrChunks {
+    uint64_t n, lo, npos, size, count;
+    uint32_t halo;
+    bool down;
+    SrChunks(uint64_t n_, uint64_t lo_, uint64_t npos_, uint32_t halo_, bool down_)
+        : n(n_), lo(lo_), npos(npos_), size(std::min<uint64_t>(sr_chunk_bytes(), (npos_ + SR_TILE - 1) / SR_TILE * SR_TILE)),
+          count((npos_ + size - 1) / size), halo(halo_), down(down_) {}
+    uint32_t positions(uint64_t c) const { return (uint32_t)std::min(size, npos - c * size); }
+    uint64_t first(uint64_t c) const { return lo + (down ? npos - c * size - positions(c) : c * size); }
+    uint64_t bytes(uint64_t c) const { return std::min<uint64_t>(positions(c) + halo, n - first(c)); }
+};
+
 #define SR_CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { err = std::string(#call " failed: ") + cudaGetErrorString(e_); \
                          return e_ == cudaErrorMemoryAllocation ? JSGPU_ENOMEM : JSGPU_ECUDA; } } while (0)
-
-template <typename T> static cudaError_t sr_grow(T*& p, size_t& cap, size_t n)
-{
-    if (n <= cap) return cudaSuccess;
-    cudaFree(p); p = nullptr; cap = 0;
-    cudaError_t e = cudaMalloc((void**)&p, n * sizeof(T));
-    if (e == cudaSuccess) cap = n;
-    return e;
-}
-
 #define SR_TRY(call) do { const int r_ = (call); if (r_ != JSGPU_OK) return r_; } while (0)
 
-// the search's streams, events and small buffers, created on the context's first search
-static int sr_open(JsSearch** ps, int device, std::string& err)
+// The context's search, made on its first use, with both slots able to take any chunk of `ch`.  The device chunk buffers
+// stay readable 64 bytes past a chunk's bytes: fv_match16 reads up to 19.
+static int sr_open(JsSearch** ps, int device, const SrChunks& ch, std::string& err)
 {
     cudaSetDevice(device);
-    if (*ps) return JSGPU_OK;
-    JsSearch* s = new JsSearch(); s->device = device;
-    *ps = s;
-    for (int i = 0; i < 2; i++) {
-        SR_CK(cudaStreamCreateWithFlags(&s->st[i], cudaStreamNonBlocking));
-        SR_CK(cudaEventCreateWithFlags(&s->copied[i], cudaEventDisableTiming));
-        SR_CK(cudaEventCreateWithFlags(&s->scanned[i], cudaEventDisableTiming));
+    if (!*ps) {
+        std::unique_ptr<JsSearch> s(new JsSearch());
+        s->device = device;
+        for (int i = 0; i < 2; i++) {
+            SR_CK(cudaStreamCreateWithFlags(&s->st[i], cudaStreamNonBlocking));
+            SR_CK(cudaEventCreateWithFlags(&s->copied[i], cudaEventDisableTiming));
+            SR_CK(cudaEventCreateWithFlags(&s->scanned[i], cudaEventDisableTiming));
+        }
+        *ps = s.release();
     }
-    size_t c0 = 0, c1 = 0, c2 = 0;
-    SR_CK(sr_grow(s->dpat, c0, (size_t)JSGPU_SEARCH_MAX_PATTERNS * 256));
-    SR_CK(sr_grow(s->dhash, c1, (size_t)(1u << SR_HBITS) / 32));
-    SR_CK(sr_grow(s->dfind, c2, 2));
-    SR_CK(cudaMallocHost((void**)&s->hfind, 2 * sizeof(uint32_t)));
+    for (int i = 0; i < 2; i++) {
+        SR_CK((*ps)->pin[i].reserve(ch.size + ch.halo));
+        SR_CK((*ps)->buf[i].reserve(ch.size + ch.halo + 64));
+    }
     return JSGPU_OK;
 }
 
-// two pinned staging buffers of at least `pin` bytes and two device chunk buffers of at least `dev` bytes
-static int sr_reserve(JsSearch* s, size_t pin, size_t dev, std::string& err)
+// Chunk c's bytes, with the overlays patched in (in installed order: the last one wins), into its slot's pinned buffer,
+// once that buffer's previous upload has left.
+static int sr_stage(JsSearch* s, const SrChunks& ch, uint64_t c, const uint8_t* data, const jsgpu_overlay* ovl, uint32_t novl,
+                    std::string& err)
 {
-    if (s->pin_cap < pin) {
-        for (int i = 0; i < 2; i++) { cudaFreeHost(s->pin[i]); s->pin[i] = nullptr; }
-        s->pin_cap = 0;
-        for (int i = 0; i < 2; i++) SR_CK(cudaMallocHost((void**)&s->pin[i], pin));
-        s->pin_cap = pin;
+    const uint64_t plo = ch.first(c), nb = ch.bytes(c);
+    uint8_t* dst = s->pin[c & 1].as<uint8_t>();
+    SR_CK(cudaEventSynchronize(s->copied[c & 1]));
+    memcpy(dst, data + plo, nb);
+    for (uint32_t k = 0; k < novl; k++) {
+        const uint64_t a = std::max<uint64_t>(ovl[k].start, plo), b = std::min<uint64_t>(ovl[k].start + ovl[k].len, plo + nb);
+        if (a < b) memcpy(dst + (a - plo), ovl[k].data + (a - ovl[k].start), b - a);
     }
-    if (s->dbuf_cap < dev) {
-        for (int i = 0; i < 2; i++) { cudaFree(s->dbuf[i]); s->dbuf[i] = nullptr; }
-        s->dbuf_cap = 0;
-        for (int i = 0; i < 2; i++) SR_CK(cudaMalloc((void**)&s->dbuf[i], dev));
-        s->dbuf_cap = dev;
-    }
+    return JSGPU_OK;
+}
+
+// Chunk c's upload from its slot's pinned buffer on the slot's stream, followed by copied[slot].
+static int sr_send(JsSearch* s, const SrChunks& ch, uint64_t c, std::string& err)
+{
+    const int sl = (int)(c & 1);
+    SR_CK(cudaMemcpyAsync(s->buf[sl].p, s->pin[sl].p, ch.bytes(c), cudaMemcpyHostToDevice, s->st[sl]));
+    SR_CK(cudaEventRecord(s->copied[sl], s->st[sl]));
     return JSGPU_OK;
 }
 
@@ -355,8 +394,6 @@ int js_search_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, 
 {
     for (uint32_t k = 0; k < npat; k++) counts[k] = 0;
     if (n == 0) return JSGPU_OK;
-    SR_TRY(sr_open(ps, device, err));
-    JsSearch* s = *ps;
 
     // patterns, their prefix hash and the reporting limits
     SrParams P; memset(&P, 0, sizeof P);
@@ -371,70 +408,63 @@ int js_search_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, 
         const uint32_t h = ((P.pre_lo[k] * 0x9E3779B1u) ^ (P.pre_hi[k] * 0x85EBCA77u)) >> (32 - SR_HBITS);
         hhash[h >> 5] |= 1u << (h & 31);
     }
-    SR_CK(cudaMemcpyAsync(s->dpat, hpat.data(), hpat.size(), cudaMemcpyHostToDevice, s->st[0]));
-    SR_CK(cudaMemcpyAsync(s->dhash, hhash.data(), hhash.size() * 4, cudaMemcpyHostToDevice, s->st[0]));
+    const SrChunks ch(n, 0, n, P.maxlen - 1, false);          // a match belongs to the chunk it starts in
+    SR_TRY(sr_open(ps, device, ch, err));
+    JsSearch* s = *ps;
+    const uint32_t tiles = (uint32_t)(ch.size / SR_TILE);
+    for (int i = 0; i < 2; i++) { SR_CK(s->sum[i].reserve((size_t)tiles * npat * 4)); SR_CK(s->off[i].reserve((size_t)tiles * npat * 4)); }
+    SR_CK(s->res.reserve(ch.count * npat * 2 * 4));
+    SR_CK(s->pat.reserve(hpat.size()));
+    SR_CK(s->hash.reserve(hhash.size() * 4));
+    SR_CK(cudaMemcpyAsync(s->pat.p, hpat.data(), hpat.size(), cudaMemcpyHostToDevice, s->st[0]));
+    SR_CK(cudaMemcpyAsync(s->hash.p, hhash.data(), hhash.size() * 4, cudaMemcpyHostToDevice, s->st[0]));
     SR_CK(cudaStreamSynchronize(s->st[0]));
-
-    const uint64_t chunk = std::min<uint64_t>(sr_chunk_bytes(), (n + SR_TILE - 1) / SR_TILE * SR_TILE);
-    const uint32_t nchunks = (uint32_t)((n + chunk - 1) / chunk);
-    const uint32_t tiles = (uint32_t)(chunk / SR_TILE);
-    const size_t span = chunk + P.maxlen - 1;                 // bytes uploaded per chunk
-    SR_TRY(sr_reserve(s, span, span, err));
-    const size_t tneed = (size_t)tiles * npat;
-    if (s->tile_cap < tneed) {
-        for (int i = 0; i < 2; i++) { cudaFree(s->dsum[i]); cudaFree(s->doff[i]); s->dsum[i] = s->doff[i] = nullptr; }
-        s->tile_cap = 0;
-        for (int i = 0; i < 2; i++) { SR_CK(cudaMalloc((void**)&s->dsum[i], tneed * 4)); SR_CK(cudaMalloc((void**)&s->doff[i], tneed * 4)); }
-        s->tile_cap = tneed;
-    }
-    SR_CK(sr_grow(s->dres, s->res_cap, (size_t)nchunks * npat * 2));
 
     int occ = 0;
     SR_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_search_tiles<false>, SR_THREADS, 0));
     const uint32_t grid = std::max(1u, std::min<uint32_t>(tiles, (uint32_t)(std::max(occ, 1) * sm_count)));
     SrEmit none; memset(&none, 0, sizeof none);
 
-    // stage chunk c into slot c & 1 and search it; `scan_after` orders the summary chain across the two streams
-    int resident = -1;
-    auto run_chunk = [&](uint32_t c, bool emit, const SrEmit& em, int prev_slot_scan) -> int {
+    // chunk c on slot c & 1: uploaded unless it is still there, summarised, and scanned after chunk c - 1's scan
+    uint64_t resident = ~0ull;
+    auto run_chunk = [&](uint32_t c, bool emit, const SrEmit& em) -> int {
         const int sl = c & 1;
-        const uint64_t c0 = (uint64_t)c * chunk, valid = std::min<uint64_t>(span, n - c0);
-        if (resident != (int)c) {
-            SR_CK(cudaEventSynchronize(s->copied[sl]));       // the pinned buffer's previous upload has left
-            memcpy(s->pin[sl], data + c0, valid);
-            SR_CK(cudaMemcpyAsync(s->dbuf[sl], s->pin[sl], valid, cudaMemcpyHostToDevice, s->st[sl]));
-            SR_CK(cudaEventRecord(s->copied[sl], s->st[sl]));
-            resident = (int)c;
+        if (resident != c) {
+            SR_TRY(sr_stage(s, ch, c, data, nullptr, 0, err));
+            SR_TRY(sr_send(s, ch, c, err));
+            resident = c;
         }
-        const uint32_t nt = (uint32_t)std::min<uint64_t>(tiles, (n - c0 + SR_TILE - 1) / SR_TILE);
-        k_search_tiles<false><<<std::min(grid, nt), SR_THREADS, 0, s->st[sl]>>>(s->dbuf[sl], c0, valid, nt, s->dpat, s->dhash, P,
-                                                                                s->dsum[sl], nullptr, none, nullptr);
-        if (prev_slot_scan >= 0) SR_CK(cudaStreamWaitEvent(s->st[sl], s->scanned[prev_slot_scan], 0));
-        k_search_scan<<<npat, 1024, 0, s->st[sl]>>>(s->dsum[sl], nt, s->doff[sl], s->dres, c, npat);
+        const uint64_t c0 = ch.first(c), valid = ch.bytes(c);
+        const uint32_t nt = (ch.positions(c) + SR_TILE - 1) / SR_TILE;
+        const uint8_t* const buf = s->buf[sl].as<uint8_t>();
+        uint32_t* const sum = s->sum[sl].as<uint32_t>();
+        uint32_t* const off = s->off[sl].as<uint32_t>();
+        k_search_tiles<false><<<std::min(grid, nt), SR_THREADS, 0, s->st[sl]>>>(buf, c0, valid, nt, s->pat.as<uint8_t>(),
+                                                                                s->hash.as<uint32_t>(), P, sum, nullptr, none, nullptr);
+        if (c) SR_CK(cudaStreamWaitEvent(s->st[sl], s->scanned[sl ^ 1], 0));
+        k_search_scan<<<npat, 1024, 0, s->st[sl]>>>(sum, nt, off, s->res.as<uint32_t>(), c, npat);
         SR_CK(cudaEventRecord(s->scanned[sl], s->st[sl]));
         if (emit)
-            k_search_tiles<true><<<std::min(grid, nt), SR_THREADS, 0, s->st[sl]>>>(s->dbuf[sl], c0, valid, nt, s->dpat, s->dhash, P,
-                                                                                   s->dsum[sl], s->doff[sl], em, s->dout);
+            k_search_tiles<true><<<std::min(grid, nt), SR_THREADS, 0, s->st[sl]>>>(buf, c0, valid, nt, s->pat.as<uint8_t>(),
+                                                                                   s->hash.as<uint32_t>(), P, sum, off, em,
+                                                                                   s->out.as<uint32_t>());
         SR_CK(cudaGetLastError());
         return JSGPU_OK;
     };
 
     // pass 1: counts per chunk and pattern
-    for (uint32_t c = 0; c < nchunks; c++) {
-        int r = run_chunk(c, false, none, c ? (int)((c - 1) & 1) : -1);
-        if (r) return r;
-    }
-    std::vector<uint32_t> res((size_t)nchunks * npat * 2);
+    for (uint32_t c = 0; c < ch.count; c++) SR_TRY(run_chunk(c, false, none));
+    std::vector<uint32_t> res(ch.count * npat * 2);
     SR_CK(cudaStreamSynchronize(s->st[0])); SR_CK(cudaStreamSynchronize(s->st[1]));
-    SR_CK(cudaMemcpy(res.data(), s->dres, res.size() * 4, cudaMemcpyDeviceToHost));
-    for (uint32_t c = 0; c < nchunks; c++) for (uint32_t k = 0; k < npat; k++) counts[k] += res[2 * ((size_t)c * npat + k)];
+    SR_CK(cudaMemcpy(res.data(), s->res.p, res.size() * 4, cudaMemcpyDeviceToHost));
+    for (uint32_t c = 0; c < ch.count; c++) for (uint32_t k = 0; k < npat; k++) counts[k] += res[2 * ((size_t)c * npat + k)];
 
     // pass 2: chunks with positions inside `cap`, written in place (pattern k's list follows pattern k-1's)
     if (cap && pos) {
         std::vector<uint64_t> first(npat), run(npat, 0);      // global index of pattern k's first position; its positions before chunk c
         uint64_t acc = 0;
         for (uint32_t k = 0; k < npat; k++) { first[k] = acc; acc += counts[k]; }
-        for (uint32_t c = 0; c < nchunks; c++) {
+        for (uint32_t c = 0; c < ch.count; c++) {
             SrEmit em; memset(&em, 0, sizeof em);
             uint64_t total = 0;
             for (uint32_t k = 0; k < npat; k++) {
@@ -443,12 +473,11 @@ int js_search_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, 
                 em.lim[k] = (uint32_t)keep; em.base[k] = (uint32_t)total; total += keep;
             }
             if (total) {
-                SR_CK(sr_grow(s->dout, s->out_cap, (size_t)total));
-                int r = run_chunk(c, true, em, c ? (int)((c - 1) & 1) : -1);
-                if (r) return r;
+                SR_CK(s->out.reserve(total * 4));
+                SR_TRY(run_chunk(c, true, em));
                 SR_CK(cudaStreamSynchronize(s->st[c & 1]));
                 std::vector<uint32_t> h(total);
-                SR_CK(cudaMemcpy(h.data(), s->dout, total * 4, cudaMemcpyDeviceToHost));
+                SR_CK(cudaMemcpy(h.data(), s->out.p, total * 4, cudaMemcpyDeviceToHost));
                 for (uint32_t k = 0; k < npat; k++)
                     if (em.lim[k]) memcpy(pos + first[k] + run[k], h.data() + em.base[k], (size_t)em.lim[k] * 4);
             }
@@ -464,8 +493,6 @@ int js_search_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, 
 // value, one position at a time, forward from start + 1 or backward from start - 1, and stops at the first match.  Here the
 // positions whose bytes all lie inside the file are searched on the device, chunk by chunk in search order; the few that
 // read past the end of the file (as 0, WindowBuf.cpp:704-711) are tested on the host.
-#define FV_THREADS 256
-#define FV_TILE    (FV_THREADS * 16)     // 16 consecutive positions per thread
 
 // Positions 0 .. npos-1 of one chunk: buf holds their npos + len - 1 bytes and is readable up to 20 bytes past the last
 // 16-byte group.  A position matches when its four bytes, little-endian and masked to len bytes, equal `pat`.
@@ -487,18 +514,18 @@ __device__ __forceinline__ uint32_t fv_match16(const uint8_t* __restrict__ buf, 
 }
 
 // res receives the lowest match (forward) or the highest match + 1 (reverse) if it beats what is there.
-__global__ void __launch_bounds__(FV_THREADS)
+__global__ void __launch_bounds__(SR_THREADS)
 k_find_value(const uint8_t* __restrict__ buf, uint32_t npos, uint32_t pat, uint32_t mask, int forward, uint32_t* __restrict__ res)
 {
     __shared__ uint32_t s_best;                              // forward: lowest match, ~0 for none; reverse: highest + 1, 0 for none
     const uint32_t tid = threadIdx.x, lane = tid & 31, none = forward ? 0xFFFFFFFFu : 0u;
     if (tid == 0) s_best = none;
     __syncthreads();
-    const uint32_t ntiles = (npos + FV_TILE - 1) / FV_TILE;
+    const uint32_t ntiles = (npos + SR_TILE - 1) / SR_TILE;
     // tiles in search order, so that a CTA can stop at its first tile with a match
     for (uint32_t i = blockIdx.x; i < ntiles; i += gridDim.x) {
         const uint32_t t = forward ? i : ntiles - 1 - i;
-        const uint32_t p0 = t * FV_TILE + 16 * tid;
+        const uint32_t p0 = t * SR_TILE + 16 * tid;
         const uint32_t m = fv_match16(buf, p0, npos, pat, mask);
         const uint32_t vote = __ballot_sync(0xffffffffu, m != 0);
         if (vote && lane == (uint32_t)(forward ? __ffs(vote) - 1 : 31 - __clz(vote))) {
@@ -559,49 +586,33 @@ int js_find_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, ui
     }
 
     if (hi >= lo) {
-        SR_TRY(sr_open(ps, device, err));
+        const SrChunks ch(n, (uint64_t)lo, (uint64_t)(hi - lo + 1), len - 1, !forward);   // the halo bytes lie in the file
+        SR_TRY(sr_open(ps, device, ch, err));
         JsSearch* s = *ps;
-        const uint64_t range = (uint64_t)(hi - lo + 1);
-        const uint64_t chunk = std::min<uint64_t>(sr_chunk_bytes(), (range + FV_TILE - 1) / FV_TILE * FV_TILE);
-        const uint64_t nchunks = (range + chunk - 1) / chunk;
-        SR_TRY(sr_reserve(s, chunk + 3, chunk + 64, err));
+        SR_CK(s->find.reserve(2 * 4));
+        SR_CK(s->hfind.reserve(2 * 4));
+        uint32_t* const dres = s->find.as<uint32_t>();
+        uint32_t* const hres = s->hfind.as<uint32_t>();
         int occ = 0;
-        SR_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_find_value, FV_THREADS, 0));
+        SR_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_find_value, SR_THREADS, 0));
         const uint32_t grid_max = (uint32_t)(std::max(occ, 1) * sm_count);
         const uint32_t pat = __builtin_bswap32(value) >> (32 - 8 * len);      // the bytes in file order, little-endian
-        // chunk c in search order: positions [plo, phi], bytes [plo, phi + len - 1] (its len - 1 halo bytes lie in the file)
-        auto bounds = [&](uint64_t c, uint64_t& plo, uint64_t& phi) {
-            if (forward) { plo = (uint64_t)lo + c * chunk; phi = std::min<uint64_t>((uint64_t)hi, plo + chunk - 1); }
-            else         { phi = (uint64_t)hi - c * chunk; plo = phi + 1 > (uint64_t)lo + chunk ? phi + 1 - chunk : (uint64_t)lo; }
-        };
-        auto stage = [&](uint64_t c) {
-            uint64_t plo, phi; bounds(c, plo, phi);
-            const uint64_t nb = phi - plo + len;
-            uint8_t* dst = s->pin[c & 1];
-            memcpy(dst, data + plo, nb);
-            for (uint32_t k = 0; k < novl; k++) {                  // installed order: the last overlay wins
-                const uint64_t a = std::max<uint64_t>(ovl[k].start, plo), b = std::min<uint64_t>(ovl[k].start + ovl[k].len, plo + nb);
-                if (a < b) memcpy(dst + (a - plo), ovl[k].data + (a - ovl[k].start), b - a);
-            }
-        };
         // The host stages chunk c + 1 while the device searches chunk c; chunk c + 1 goes to the device only if c has no match.
-        stage(0);
-        for (uint64_t c = 0; c < nchunks; c++) {
+        SR_TRY(sr_stage(s, ch, 0, data, ovl, novl, err));
+        for (uint64_t c = 0; c < ch.count; c++) {
             const int sl = (int)(c & 1);
-            uint64_t plo, phi; bounds(c, plo, phi);
-            const uint32_t npos = (uint32_t)(phi - plo + 1);
-            SR_CK(cudaMemcpyAsync(s->dbuf[sl], s->pin[sl], npos + len - 1, cudaMemcpyHostToDevice, s->st[sl]));
-            SR_CK(cudaMemsetAsync(s->dfind + sl, forward ? 0xFF : 0, 4, s->st[sl]));
-            const uint32_t grid = std::max(1u, std::min(grid_max, (npos + FV_TILE - 1) / FV_TILE));
-            k_find_value<<<grid, FV_THREADS, 0, s->st[sl]>>>(s->dbuf[sl], npos, pat, mask, forward, s->dfind + sl);
+            const uint32_t npos = ch.positions(c);
+            SR_TRY(sr_send(s, ch, c, err));
+            SR_CK(cudaMemsetAsync(dres + sl, forward ? 0xFF : 0, 4, s->st[sl]));
+            const uint32_t grid = std::max(1u, std::min(grid_max, (npos + SR_TILE - 1) / SR_TILE));
+            k_find_value<<<grid, SR_THREADS, 0, s->st[sl]>>>(s->buf[sl].as<uint8_t>(), npos, pat, mask, forward, dres + sl);
             SR_CK(cudaGetLastError());
-            SR_CK(cudaMemcpyAsync(s->hfind + sl, s->dfind + sl, 4, cudaMemcpyDeviceToHost, s->st[sl]));
-            SR_CK(cudaEventRecord(s->copied[sl], s->st[sl]));
-            if (c + 1 < nchunks) stage(c + 1);                    // the other slot's chunk finished in the previous round
-            SR_CK(cudaEventSynchronize(s->copied[sl]));
-            const uint32_t r = s->hfind[sl];
+            SR_CK(cudaMemcpyAsync(hres + sl, dres + sl, 4, cudaMemcpyDeviceToHost, s->st[sl]));
+            if (c + 1 < ch.count) SR_TRY(sr_stage(s, ch, c + 1, data, ovl, novl, err));
+            SR_CK(cudaStreamSynchronize(s->st[sl]));
+            const uint32_t r = hres[sl];
             if (forward ? r != 0xFFFFFFFFu : r != 0u) {
-                *found = 1; *found_pos = plo + (forward ? r : r - 1);
+                *found = 1; *found_pos = ch.first(c) + (forward ? r : r - 1);
                 return JSGPU_OK;
             }
         }
@@ -615,23 +626,23 @@ int js_find_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, ui
 // each CTA's run of consecutive tiles, k_find_all_scan turns the counts into output indices from the running total kept on
 // the device, and k_find_all<true> writes the positions in file order.  CTA b owns tiles [b * per, (b + 1) * per).
 template <bool EMIT>
-__global__ void __launch_bounds__(FV_THREADS)
+__global__ void __launch_bounds__(SR_THREADS)
 k_find_all(const uint8_t* __restrict__ buf, uint32_t npos, uint32_t pat, uint32_t mask, uint32_t per, uint32_t chunk_pos,
            uint32_t* __restrict__ cta /*[2][gridDim.x]: counts, then first output index*/, uint32_t* __restrict__ out, uint64_t cap)
 {
-    __shared__ uint32_t s_w[FV_THREADS / 32];
+    __shared__ uint32_t s_w[SR_THREADS / 32 + 1];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t ntiles = (npos + FV_TILE - 1) / FV_TILE;
+    const uint32_t ntiles = (npos + SR_TILE - 1) / SR_TILE;
     const uint32_t t0 = blockIdx.x * per, t1 = min(ntiles, t0 + per);
     if (!EMIT) {
         uint32_t c = 0;
-        for (uint32_t t = t0; t < t1; t++) c += __popc(fv_match16(buf, t * FV_TILE + 16 * tid, npos, pat, mask));
+        for (uint32_t t = t0; t < t1; t++) c += __popc(fv_match16(buf, t * SR_TILE + 16 * tid, npos, pat, mask));
         c = __reduce_add_sync(0xffffffffu, c);
         if (lane == 0) s_w[warp] = c;
         __syncthreads();
         if (tid == 0) {
             uint32_t sum = 0;
-            for (int k = 0; k < FV_THREADS / 32; k++) sum += s_w[k];
+            for (int k = 0; k < SR_THREADS / 32; k++) sum += s_w[k];
             cta[blockIdx.x] = sum;
         }
         return;
@@ -639,24 +650,10 @@ k_find_all(const uint8_t* __restrict__ buf, uint32_t npos, uint32_t pat, uint32_
     uint32_t j = cta[gridDim.x + blockIdx.x];                // this CTA's first output index
     if (cta[blockIdx.x] == 0 || j >= cap) return;
     for (uint32_t t = t0; t < t1 && j < cap; t++) {
-        uint32_t m = fv_match16(buf, t * FV_TILE + 16 * tid, npos, pat, mask);
-        const uint32_t c = __popc(m);
-        uint32_t inc = c;                                     // inclusive scan over the warp, then over the warps
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xffffffffu, inc, d);
-            if (lane >= (uint32_t)d) inc += v;
-        }
-        __syncthreads();                                      // the previous tile is done with s_w
-        if (lane == 31) s_w[warp] = inc;
-        __syncthreads();
-        uint32_t before = 0, tot = 0;
-#pragma unroll
-        for (int k = 0; k < FV_THREADS / 32; k++) { const uint32_t v = s_w[k]; before += (uint32_t)k < warp ? v : 0u; tot += v; }
-        uint64_t o = (uint64_t)j + before + inc - c;
-        const uint32_t p = chunk_pos + t * FV_TILE + 16 * tid;
+        uint32_t m = fv_match16(buf, t * SR_TILE + 16 * tid, npos, pat, mask);
+        uint64_t o = block_scan<SR_THREADS>((uint32_t)__popc(m), 0u, sr_add, j, s_w);   // advances j past the tile
+        const uint32_t p = chunk_pos + t * SR_TILE + 16 * tid;
         while (m && o < cap) { out[o++] = p + (uint32_t)__ffs((int)m) - 1; m &= m - 1; }
-        j += tot;
     }
 }
 
@@ -664,28 +661,14 @@ k_find_all(const uint8_t* __restrict__ buf, uint32_t npos, uint32_t pat, uint32_
 __global__ void __launch_bounds__(1024)
 k_find_all_scan(uint32_t* __restrict__ cta, uint32_t ncta, uint32_t* __restrict__ total)
 {
-    __shared__ uint32_t s_w[32], s_run;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) s_run = *total;
+    __shared__ uint32_t s_w[33];
+    uint32_t run = *total;
     for (uint32_t b0 = 0; b0 < ncta; b0 += 1024) {
-        __syncthreads();
-        const uint32_t b = b0 + tid, c = b < ncta ? cta[b] : 0u;
-        uint32_t inc = c;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xffffffffu, inc, d);
-            if (lane >= (uint32_t)d) inc += v;
-        }
-        if (lane == 31) s_w[warp] = inc;
-        __syncthreads();
-        uint32_t before = 0, tot = 0;
-        for (uint32_t k = 0; k < 32; k++) { const uint32_t v = s_w[k]; before += k < warp ? v : 0u; tot += v; }
-        if (b < ncta) cta[ncta + b] = s_run + before + inc - c;
-        __syncthreads();
-        if (tid == 0) s_run += tot;
+        const uint32_t b = b0 + threadIdx.x;
+        const uint32_t o = block_scan<1024>(b < ncta ? cta[b] : 0u, 0u, sr_add, run, s_w);
+        if (b < ncta) cta[ncta + b] = o;
     }
-    __syncthreads();
-    if (tid == 0) *total = s_run;
+    if (threadIdx.x == 0) *total = run;
 }
 
 int js_find_all_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, uint64_t n, uint32_t value, uint32_t len,
@@ -694,44 +677,35 @@ int js_find_all_run(JsSearch** ps, int device, int sm_count, const uint8_t* data
     *count = 0;
     const uint32_t mask = len == 4 ? 0xFFFFFFFFu : (1u << (8 * len)) - 1u;
     if (n < len || (value & ~mask)) return JSGPU_OK;         // no position, or a value wider than len bytes
-    SR_TRY(sr_open(ps, device, err));
+    const SrChunks ch(n, 0, n - len + 1, len - 1, false);
+    SR_TRY(sr_open(ps, device, ch, err));
     JsSearch* s = *ps;
-    const uint64_t npos_all = n - len + 1;
-    const uint64_t chunk = std::min<uint64_t>(sr_chunk_bytes(), (npos_all + FV_TILE - 1) / FV_TILE * FV_TILE);
-    const uint64_t nchunks = (npos_all + chunk - 1) / chunk;
-    SR_TRY(sr_reserve(s, chunk + 3, chunk + 64, err));
     int occ = 0;
-    SR_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_find_all<true>, FV_THREADS, 0));
+    SR_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_find_all<true>, SR_THREADS, 0));
     const uint32_t grid_max = (uint32_t)(std::max(occ, 1) * sm_count);
-    if (s->fa_cap < 2 * (size_t)grid_max) {
-        for (int i = 0; i < 2; i++) { cudaFree(s->dfa[i]); s->dfa[i] = nullptr; }
-        s->fa_cap = 0;
-        for (int i = 0; i < 2; i++) SR_CK(cudaMalloc((void**)&s->dfa[i], 2 * (size_t)grid_max * 4));
-        s->fa_cap = 2 * (size_t)grid_max;
-    }
-    const uint64_t keep = std::min<uint64_t>(cap, npos_all);  // positions the device list can hold
-    if (keep) SR_CK(sr_grow(s->dout, s->out_cap, (size_t)keep));
+    for (int i = 0; i < 2; i++) SR_CK(s->cta[i].reserve(2 * (size_t)grid_max * 4));
+    const uint64_t keep = std::min<uint64_t>(cap, ch.npos);   // positions the device list can hold
+    if (keep) SR_CK(s->out.reserve(keep * 4));
+    SR_CK(s->total.reserve(4));
     const uint32_t pat = __builtin_bswap32(value) >> (32 - 8 * len);      // the bytes in file order, little-endian
-    uint32_t* const total = s->dfind;                                     // the running count (the value search's result word)
+    uint32_t* const total = s->total.as<uint32_t>();
     SR_CK(cudaMemsetAsync(total, 0, 4, s->st[0]));
     SR_CK(cudaEventRecord(s->scanned[1], s->st[0]));                      // chunk 0's scan follows the reset
 
-    for (uint64_t c = 0; c < nchunks; c++) {
+    for (uint64_t c = 0; c < ch.count; c++) {
         const int sl = (int)(c & 1);
-        const uint64_t plo = c * chunk;
-        const uint32_t npos = (uint32_t)std::min<uint64_t>(chunk, npos_all - plo);
-        SR_CK(cudaEventSynchronize(s->copied[sl]));           // the pinned buffer's previous upload has left
-        memcpy(s->pin[sl], data + plo, npos + len - 1);
-        SR_CK(cudaMemcpyAsync(s->dbuf[sl], s->pin[sl], npos + len - 1, cudaMemcpyHostToDevice, s->st[sl]));
-        SR_CK(cudaEventRecord(s->copied[sl], s->st[sl]));
-        const uint32_t ntiles = (npos + FV_TILE - 1) / FV_TILE;
+        const uint32_t npos = ch.positions(c), plo = (uint32_t)ch.first(c);
+        SR_TRY(sr_stage(s, ch, c, data, nullptr, 0, err));
+        SR_TRY(sr_send(s, ch, c, err));
+        const uint8_t* const buf = s->buf[sl].as<uint8_t>();
+        uint32_t* const cta = s->cta[sl].as<uint32_t>();
+        const uint32_t ntiles = (npos + SR_TILE - 1) / SR_TILE;
         const uint32_t grid = std::max(1u, std::min(grid_max, ntiles)), per = (ntiles + grid - 1) / grid;
-        k_find_all<false><<<grid, FV_THREADS, 0, s->st[sl]>>>(s->dbuf[sl], npos, pat, mask, per, (uint32_t)plo, s->dfa[sl], nullptr, 0);
+        k_find_all<false><<<grid, SR_THREADS, 0, s->st[sl]>>>(buf, npos, pat, mask, per, plo, cta, nullptr, 0);
         SR_CK(cudaStreamWaitEvent(s->st[sl], s->scanned[sl ^ 1], 0));  // the previous chunk has advanced the total
-        k_find_all_scan<<<1, 1024, 0, s->st[sl]>>>(s->dfa[sl], grid, total);
+        k_find_all_scan<<<1, 1024, 0, s->st[sl]>>>(cta, grid, total);
         SR_CK(cudaEventRecord(s->scanned[sl], s->st[sl]));
-        if (keep)
-            k_find_all<true><<<grid, FV_THREADS, 0, s->st[sl]>>>(s->dbuf[sl], npos, pat, mask, per, (uint32_t)plo, s->dfa[sl], s->dout, keep);
+        if (keep) k_find_all<true><<<grid, SR_THREADS, 0, s->st[sl]>>>(buf, npos, pat, mask, per, plo, cta, s->out.as<uint32_t>(), keep);
         SR_CK(cudaGetLastError());
     }
     SR_CK(cudaStreamSynchronize(s->st[0])); SR_CK(cudaStreamSynchronize(s->st[1]));
@@ -739,6 +713,6 @@ int js_find_all_run(JsSearch** ps, int device, int sm_count, const uint8_t* data
     SR_CK(cudaMemcpy(&tot, total, 4, cudaMemcpyDeviceToHost));
     *count = tot;
     const uint64_t got = std::min<uint64_t>(tot, keep);
-    if (got) SR_CK(cudaMemcpy(pos, s->dout, got * 4, cudaMemcpyDeviceToHost));
+    if (got) SR_CK(cudaMemcpy(pos, s->out.p, got * 4, cudaMemcpyDeviceToHost));
     return JSGPU_OK;
 }

@@ -400,7 +400,7 @@ class BatchDecoder:
         """jsgpu_search_bytes: every position the reference's repeated BufSearchX loop reports for each pattern (8..256 bytes,
         at most 32) in `data` (bytes or a uint8 array).  Returns (counts uint64 [npat], [positions uint32 array per pattern]);
         with `cap`, at most cap positions are returned in all (counts stay complete)."""
-        buf = data if isinstance(data, np.ndarray) else np.frombuffer(bytes(data), np.uint8)
+        buf = _u8(data)
         pats = [np.frombuffer(bytes(p), np.uint8) for p in patterns]
         cat = np.concatenate(pats) if pats else np.zeros(0, np.uint8)
         lens = np.array([p.size for p in pats], np.uint32)
@@ -418,7 +418,7 @@ class BatchDecoder:
     def find_value(self, data, start, value, length, forward=True, overlays=()):
         """jsgpu_find_value: what CwindowBuf::BufSearch(start, value, length, forward) returns over `data` (bytes or a uint8
         array) with `overlays` [(start, bytes), ...] applied, the last one winning: (found, position)."""
-        buf = data if isinstance(data, np.ndarray) else np.frombuffer(bytes(data), np.uint8)
+        buf = _u8(data)
         keep = [np.frombuffer(bytes(b), np.uint8) for _, b in overlays]
         ov = (B.jsgpu_overlay * max(len(keep), 1))(*[B.jsgpu_overlay(int(o), a.size, a.ctypes.data) for (o, _), a in zip(overlays, keep)])
         found, pos = C.c_int(0), C.c_uint64(0)

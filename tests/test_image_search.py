@@ -259,6 +259,31 @@ def test_gpu_unaligned_host_buffers(built, monkeypatch):
 
 
 @pytest.mark.gpu
+def test_gpu_strided_views_search_their_own_bytes(built):
+    """A strided uint8 view is searched element by element, not as the memory under its first elements: find_value and
+    search_bytes give what they give for its contiguous copy."""
+    from jpegsnoop_b200 import BatchDecoder
+    bd = BatchDecoder()
+    cont, offs = container(9)
+    pat = np.random.default_rng(9).integers(0, 256, 64, dtype=np.uint8)
+    planted = [100, len(cont) // 2, len(cont) - 300]
+    raw = np.zeros(2 * len(cont), np.uint8)                     # the view's bytes interleaved with zeros in memory
+    view = raw[::2]
+    view[:] = np.frombuffer(cont, np.uint8)
+    for p in planted:
+        view[p:p + pat.size] = pat
+    flat = view.copy()
+    assert not view.flags.c_contiguous
+    counts, (pos,) = bd.search_bytes(view, [pat.tobytes()])
+    counts0, (pos0,) = bd.search_bytes(flat, [pat.tobytes()])
+    assert counts.tolist() == counts0.tolist() == [len(planted)]
+    assert pos.tolist() == pos0.tolist() == planted
+    for s in (0, offs[1], offs[3] + 1, len(cont)):
+        for f in (True, False):
+            assert bd.find_value(view, s, SOI3, 3, f) == bd.find_value(flat, s, SOI3, 3, f) == F.bufsearch_model(flat, s, SOI3, 3, f)
+
+
+@pytest.mark.gpu
 def test_gpu_size_limit(built):
     from jpegsnoop_b200 import BatchDecoder, CimgDecode, JsgpuError
     big = np.zeros(1 << 32, np.uint8)                          # pages never touched
