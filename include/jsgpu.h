@@ -426,6 +426,23 @@ int jsgpu_find_value(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, uint64_t s
 int jsgpu_find_all(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, uint32_t value, uint32_t len, uint64_t* count, uint32_t* pos,
                    uint64_t cap);
 
+/* --- the markers of Extract embedded JPEG / Extract All (JPEGsnoopCore.cpp:913-1088) ---------------------------------------
+ * One streaming pass that lists, in ascending order:
+ *   soi_pos   every p in [0, n - 3] whose bytes are FF D8 FF: the list jsgpu_find_all(value 0xFFD8FF, len 3) returns, whose
+ *             positions from 1 on are the frame starts Extract All's chain of BufSearch calls visits;
+ *   term_pos  every PASS-1 scan terminator (CjfifDecode::DecodeMarker, JfifDecode.cpp:5194-5265): p in [0, n - 2] with
+ *             byte p == FF and byte p + 1 neither 00 nor D0..D7.  The byte after a stuffed or RST FF is never FF, so the end
+ *             of a scan starting at s is the first terminator >= s, whatever the scan holds; with none, the scan runs out of
+ *             file ("Ran out of buffer before EOI").  An FF in the last byte ends nothing: Buf() reads the byte past the end
+ *             of the file as 0.
+ * Both are read with `noverlays` overlays applied as jsgpu_find_value applies them (bytes an overlay puts past the end of the
+ * file are not searched).  *nsoi / *nterm receive complete counts; soi_pos / term_pos receive at most soi_cap / term_cap
+ * positions.  Each chunk (JSGPU_SEARCH_CHUNK_BYTES) is uploaded once with its next two bytes, so a terminator or an SOI on a
+ * chunk's last positions is decided there.  Files of 2^32 bytes or more are refused (JSGPU_EINVAL).  The batch of the
+ * context is left untouched.  Synchronous. */
+int jsgpu_find_markers(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, const jsgpu_overlay* overlays, uint32_t noverlays,
+                       uint32_t* soi_pos, uint64_t soi_cap, uint64_t* nsoi, uint32_t* term_pos, uint64_t term_cap, uint64_t* nterm);
+
 /* Pinned host memory helpers (for callers that want true async copies). */
 void* jsgpu_host_alloc(uint64_t bytes);
 void  jsgpu_host_free(void* p);

@@ -114,6 +114,37 @@ int    jsimg_img_search(jsimg*, uint64_t start, int fwd, int quiet, int* found, 
 #define JSIMG_OFFSET_POS   3
 int    jsimg_decode_offset_mode(jsimg*, const uint8_t* data, uint64_t n, int mode, uint64_t pos, int quiet, uint64_t* pos_used);
 
+/* Tools -> Extract embedded JPEG and its Extract All mode (JPEGsnoopCore.cpp:913-1088; CjfifDecode::ExportJpegPrepare /
+ * ExportJpegDo, JfifDecode.cpp:7544-7797) over the installed file and overlays.  One GPU pass (jsgpu_find_markers) lists the
+ * FF D8 FF candidates and the PASS-1 scan terminators; the host then walks each frame's markers from its start to the EOI as
+ * ProcessFile does (every scan skipped to its first terminator), and copies the frame out of the caller's buffer.  Nothing is
+ * decoded.  The bytes are the reference's, quirks included:
+ *   - [start, first SOS) and [first SOS, end) are each copied by a loop that stops one byte short of a part of
+ *     k * 131072 + 1 bytes (for the second part that byte is the EOI's D9), and writes nothing of a 1-byte part;
+ *   - FORCE_SOI writes FF D8 only when the walk met no SOI; FORCE_EOI appends FF D9 always, after a real EOI too;
+ *   - with no EOI, FORCE_EOI or IGNORE_EOI end the frame at the end of the file (otherwise the export is refused);
+ *   - DHT_AVI inserts the 0x1A4-byte Annex K DHT segment before the first SOS, whatever the frame holds;
+ *   - OVERLAY copies the bytes through the overlays; the walk always reads through them.
+ * The log receives the reference's lines: the "*** Exporting JPEG ***" header, "Exporting from / to", the Prepare errors and
+ * warnings, "Forcing SOI/EOI Marker", "Inserting standard AVI DHT huffman table", "Export done", "Can't overwrite source
+ * file" when out_path equals src_name (the names are compared, as the reference does).  Files of 2^32 bytes or more are
+ * refused (JSGPU_EINVAL, one error line).
+ * jsimg_export_jpeg: the frame at `pos` (which need not hold an SOI) into out_path; 1 written, 0 refused, or a negative
+ *   JSGPU_E* code from the search.
+ * jsimg_extract_all: frames from offset 0, then from each FF D8 FF after the previous start (thumbnails nested in an APP1
+ *   included), written to root.000001.jpg, root.000002.jpg, ... where root is out_name up to its last '.'.  A frame the
+ *   Prepare step refuses takes no number.  offsets / numbers receive, for the first `cap` frames analysed, the frame's offset
+ *   and its file's number (0: not written).  Returns the number of frames analysed, JSGPU_EINVAL after "ERROR: Invalid
+ *   filename" when out_name has no '.', or a negative JSGPU_E* code from the search.  The search runs on `ctx` when given
+ *   (a batch resident there is left untouched), else on the handle's own search context. */
+#define JSIMG_EXPORT_OVERLAY    1u
+#define JSIMG_EXPORT_FORCE_SOI  2u
+#define JSIMG_EXPORT_FORCE_EOI  4u
+#define JSIMG_EXPORT_IGNORE_EOI 8u
+#define JSIMG_EXPORT_DHT_AVI    16u
+int     jsimg_export_jpeg(jsimg*, uint64_t pos, const char* src_name, const char* out_path, unsigned flags);
+int64_t jsimg_extract_all(jsimg*, jsgpu_ctx* ctx, const char* src_name, const char* out_name, unsigned flags, uint64_t* offsets,
+                          uint32_t* numbers, uint64_t cap);
 /* log access (error convention: failures are log lines, ImgDecode.cpp:2755-2758 etc.) */
 int    jsimg_log_count(jsimg*, int kind /*0 line,1 hdr,2 warn,3 err,4 good,-1 all*/);
 const char* jsimg_log_line(jsimg*, int kind, int index);

@@ -110,7 +110,7 @@ JSGPU_SYMBOLS = [
     "jsgpu_batch_begin", "jsgpu_batch_layout", "jsgpu_batch_pools", "jsgpu_batch_upload", "jsgpu_batch_decode",
     "jsgpu_batch_download", "jsgpu_batch_stage_ms", "jsgpu_timer_start", "jsgpu_timer_stop", "jsgpu_batch_launches", "jsgpu_batch_selfsync_info", "jsgpu_batch_checksums", "jsgpu_batch_errors", "jsgpu_batch_error_events", "jsgpu_decode_batch_host",
     "jsgpu_host_alloc", "jsgpu_host_free", "jsgpu_host_copy_rate", "jsgpu_set_preview", "jsgpu_batch_preview", "jsgpu_batch_colour_stats", "jsgpu_batch_export", "jsgpu_set_detail", "jsgpu_batch_detail",
-    "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices", "jsgpu_search_bytes", "jsgpu_find_value", "jsgpu_find_all"]
+    "jsgpu_batch_detail_info", "jsgpu_batch_detail_events", "jsgpu_batch_detail_matrices", "jsgpu_search_bytes", "jsgpu_find_value", "jsgpu_find_all", "jsgpu_find_markers"]
 JSIMG_SYMBOLS = [
     "jsimg_create", "jsimg_destroy", "jsimg_config", "jsimg_set_file", "jsimg_overlay_install", "jsimg_overlay_remove_all", "jsimg_Reset", "jsimg_ResetState",
     "jsimg_SetDqtEntry", "jsimg_SetDqtTables", "jsimg_GetDqtEntry", "jsimg_SetDhtTables", "jsimg_SetDhtEntry",
@@ -122,7 +122,8 @@ JSIMG_SYMBOLS = [
     "jsimg_config_histo", "jsimg_SetPreviewMode", "jsimg_GetPreviewMode", "jsimg_SetPreviewYccOffset", "jsimg_GetPreviewYccOffset",
     "jsimg_GetStatClip", "jsimg_GetHistoRanges", "jsimg_GetCcHisto", "jsimg_GetHistoYFull", "jsimg_GetHistoDib", "jsimg_ExportTiff", "jsimg_tiff_write", "jsimg_SetDetailVlc", "jsimg_GetDetailVlc",
     "jsimg_search_dqt", "jsimg_buf_search", "jsimg_decode_jpeg_at", "jsimg_img_search", "jsimg_decode_offset_mode", "jsimg_parse_jpeg_at",
-    "jsimg_config_scan_err_max", "jsimg_ScanErrorsDisable", "jsimg_ScanErrorsEnable"]
+    "jsimg_config_scan_err_max", "jsimg_ScanErrorsDisable", "jsimg_ScanErrorsEnable",
+    "jsimg_export_jpeg", "jsimg_extract_all"]
 
 _lib = None
 
@@ -182,6 +183,9 @@ def load():
     L.jsimg_search_dqt.argtypes = [vp, vp, u64, C.c_char_p, i32, C.c_char_p]
     L.jsgpu_find_value.argtypes = [vp, vp, u64, u64, u32, u32, i32, vp, u32, C.POINTER(i32), C.POINTER(u64)]
     L.jsgpu_find_all.argtypes = [vp, vp, u64, u32, u32, C.POINTER(u64), vp, u64]
+    L.jsgpu_find_markers.argtypes = [vp, vp, u64, vp, u32, vp, u64, C.POINTER(u64), vp, u64, C.POINTER(u64)]
+    L.jsimg_export_jpeg.argtypes = [vp, u64, C.c_char_p, C.c_char_p, u32]
+    L.jsimg_extract_all.argtypes = [vp, vp, C.c_char_p, C.c_char_p, u32, vp, vp, u64]; L.jsimg_extract_all.restype = C.c_int64
     L.jsimg_buf_search.argtypes = [vp, u64, u32, u32, i32, C.POINTER(u64)]
     L.jsimg_decode_jpeg_at.argtypes = [vp, vp, u64, u64, i32]
     L.jsimg_img_search.argtypes = [vp, u64, i32, i32, C.POINTER(i32), C.POINTER(u64), C.POINTER(i32)]

@@ -4,6 +4,7 @@
 // SOF 5001-5026, DHT 3535-3600, DRI 5310-5330, SOS 5150-5164 + 5291, the AVI1 Huffman-table
 // import 4406-4426).  Everything else the reference parser does (EXIF, signatures, thumbnails,
 // logging) is out of scope (SURVEY.md §8f N1).
+#include <algorithm>
 #include <vector>
 #include "ImgDecode.h"
 #include "JfifWalk.h"
@@ -39,7 +40,7 @@ static int WalkDht(CimgDecode* pImgDec, const uint8_t* d, uint64_t q, uint64_t e
 
 // The tables of the DHT segment a Motion-JPEG frame leaves out (OpenDML AVI, "Proposed Data Chunk Format"): the T.81
 // Annex K tables in the order DC 0, DC 1, AC 0, AC 1, as the Tc/Th bytes, BITS and HUFFVAL of one DHT segment.
-static const std::vector<uint8_t>& MjpgDhtTables()
+const std::vector<uint8_t>& MjpgDhtTables()
 {
     static const std::vector<uint8_t> seg = [] {
         using namespace annex_k;
@@ -72,27 +73,72 @@ static bool App0IsAvi1(const uint8_t* d, uint64_t n, uint64_t q)
     return k == 4;
 }
 
-int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n, uint64_t nPosStart, bool* pbSof)
+// One walk for both callers.  Without pEnd it is the decode walk: the first frame's setter sequence from an SOI at nPosStart
+// to its first SOS.  With pEnd it is ProcessFile's loop to the EOI (JfifDecode.cpp:7430-7451, DecodeMarker :3783-5440),
+// recording the export state; pImgDec is then null and no setter is called.  A segment that runs past the end of the file
+// stops it there (the reference reads 0s past the end and then stops at "Early EOF").
+static int Walk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n, uint64_t nPosStart, bool* pbSof, const uint32_t* term,
+                uint64_t nterm, JfifEnd* pEnd)
 {
     unsigned unzz[64];
     for (unsigned i = 0; i < 64; i++) unzz[kJfifZigZag[i]] = i;
-    pImgDec->ResetState();
+    const bool bToEoi = pEnd != nullptr;
+    if (pImgDec) pImgDec->ResetState();
     bool bSofSeen = false;                                          // CjfifDecode::m_bImgOK (JfifDecode.cpp:96, 5030)
     if (!pbSof) pbSof = &bSofSeen;
     *pbSof = false;
-    // ProcessFile starts the marker walk at m_pAppConfig->nPosStart and every position stays absolute (JfifDecode.cpp:7338-7341)
-    if (nPosStart >= n || n - nPosStart < 4 || d[nPosStart] != 0xFF || d[nPosStart + 1] != 0xD8) return JFIFWALK_ENOTJPEG;
-    uint64_t p = nPosStart + 2;
+    auto byte = [&](uint64_t q) -> unsigned { return q < n ? d[q] : 0u; };   // Buf(): 0 past the end of the file
+    uint64_t p = nPosStart;
+    if (!bToEoi) {
+        // ProcessFile starts the marker walk at m_pAppConfig->nPosStart and every position stays absolute (JfifDecode.cpp:7338-7341)
+        if (nPosStart >= n || n - nPosStart < 4 || d[nPosStart] != 0xFF || d[nPosStart + 1] != 0xD8) return JFIFWALK_ENOTJPEG;
+        p = nPosStart + 2;
+    }
     unsigned X = 0, Y = 0, Nf = 0, P = 8, nRstInterval = 0;
     bool bRstEn = false, bSof = false;
-    while (p + 4 <= n) {
+    while (bToEoi ? p < n : p + 4 <= n) {
         if (d[p] != 0xFF) return JFIFWALK_EMARKER;
-        unsigned m = d[p + 1]; p += 2;
+        unsigned m = byte(p + 1); p += 2;
         if (m == 0xFF) { p -= 1; continue; }                       // fill byte
-        if (m == 0xD8 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) continue;
-        if (m == 0xD9) return JFIFWALK_ENOSCAN;
-        unsigned L = ((unsigned)d[p] << 8) | d[p + 1];
+        if (bToEoi) {
+            if (m == 0xD8) { pEnd->bSoi = true; continue; }
+            if (m == 0xD9) { pEnd->bEoi = true; pEnd->nPosEmbedEnd = p; return 0; }     // :5338-5342
+            // RSTn outside a scan and the markers DecodeMarker has no case for stop the walk (bRelaxedParsing off, :5350-5430)
+            const bool bKnown = (m >= 0xC0 && m <= 0xCF) || (m >= 0xDA && m <= 0xFE) || m == 0x01;
+            if (!bKnown) return JFIFWALK_EMARKER;
+        } else {
+            if (m == 0xD8 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) continue;
+            if (m == 0xD9) return JFIFWALK_ENOSCAN;
+        }
+        unsigned L = (byte(p) << 8) | byte(p + 1);
         uint64_t q = p + 2, e = p + L;
+        if (bToEoi) {
+            if (m == 0xDB) pEnd->bDqt = true;                                       // :4440
+            if (m == 0xC4 || (m == 0xE0 && App0IsAvi1(d, n, q))) pEnd->bDht = true;  // :5100, the AVI1 import :4397, 4421
+            if (m >= 0xC0 && m <= 0xCF && m != 0xC4 && m != 0xC8 && m != 0xCC) { pEnd->bSof = bSof = true; *pbSof = true; }   // :4821, 5032
+            if (m == 0xDA) {
+                pEnd->bSos = true;                                                  // :5108-5116
+                if (pEnd->nPosSos == 0) pEnd->nPosSos = p - 2;
+                if (!bSof) return JFIFWALK_EMARKER;                                 // "SOS before valid SOF defined"
+            }
+            if (e > n) return JFIFWALK_ETRUNC;
+            if (m == 0xDB) {                                                        // Pq 0..1, Tq 0..3 (:4473-4474)
+                while (q < e) {
+                    const unsigned Pq = d[q] >> 4, Tq = d[q] & 15;
+                    if (Pq > 1 || Tq > 3) return JFIFWALK_EMARKER;
+                    q += 1 + 64 * (Pq + 1);
+                }
+            }
+            if (m == 0xDA) {
+                // PASS 1 (:5194-5265): the scan ends at the first terminator at or after its start, or runs out of file
+                const uint32_t* t = std::lower_bound(term, term + nterm, e, [](uint32_t a, uint64_t b) { return a < b; });
+                if (t == term + nterm) return JFIFWALK_ETRUNC;
+                p = *t;
+                continue;
+            }
+            p = e;
+            continue;
+        }
         if (L < 2 || e > n) return JFIFWALK_ETRUNC;
         switch (m) {
         case 0xDB:                                                  // DQT
@@ -149,4 +195,15 @@ int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n, uint64_t nPosSta
         p = e;
     }
     return JFIFWALK_ENOSCAN;
+}
+
+int JfifWalk(CimgDecode* pImgDec, const uint8_t* d, uint64_t n, uint64_t nPosStart, bool* pbSof)
+{
+    return Walk(pImgDec, d, n, nPosStart, pbSof, nullptr, 0, nullptr);
+}
+
+void JfifWalkToEoi(const uint8_t* d, uint64_t n, uint64_t nPosStart, const uint32_t* term, uint64_t nterm, JfifEnd* pEnd)
+{
+    *pEnd = JfifEnd();
+    Walk(nullptr, d, n, nPosStart, nullptr, term, nterm, pEnd);
 }

@@ -3,6 +3,7 @@
 #include "ImgDecode.h"
 #include "TiffExport.h"
 #include "JfifWalk.h"
+#include "JpegExport.h"
 #include "DqtSearch.h"
 #include <cstring>
 
@@ -172,4 +173,26 @@ int jsimg_parse_jpeg_at(const uint8_t* d, uint64_t n, uint64_t pos, jsgpu_tables
     desc->scan_offset = (uint64_t)start; desc->scan_length = n - (uint64_t)start;
     return start;
 }
+}
+
+int jsimg_export_jpeg(jsimg* h, uint64_t pos, const char* src_name, const char* out_path, unsigned flags)
+{
+    std::vector<uint32_t> soi, term;
+    const int r = JpegFindMarkers(&h->log, &h->search, h->cfg.nCudaDevice, h->wbuf, soi, term);
+    if (r != JSGPU_OK) return r;
+    return JpegExportOne(&h->log, h->wbuf, term, pos, src_name ? src_name : "", out_path ? out_path : "", flags);
+}
+
+int64_t jsimg_extract_all(jsimg* h, jsgpu_ctx* ctx, const char* src_name, const char* out_name, unsigned flags, uint64_t* offsets,
+                          uint32_t* numbers, uint64_t cap)
+{
+    std::vector<uint32_t> soi, term;
+    const int r = JpegFindMarkers(&h->log, ctx ? &ctx : &h->search, h->cfg.nCudaDevice, h->wbuf, soi, term);
+    if (r != JSGPU_OK) return r;
+    std::vector<uint64_t> offs;
+    std::vector<uint32_t> nums;
+    const int64_t k = JpegExtractAll(&h->log, h->wbuf, soi, term, src_name ? src_name : "", out_name ? out_name : "", flags, offs, nums);
+    if (k < 0) return JSGPU_EINVAL;
+    for (uint64_t i = 0; i < std::min<uint64_t>(cap, offs.size()); i++) { offsets[i] = offs[i]; numbers[i] = nums[i]; }
+    return k;
 }

@@ -1165,6 +1165,21 @@ int jsgpu_find_all(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, uint32_t val
     return js_find_all_run(&ctx->search, ctx->device, ctx->sm_count, data, n, value, len, count, pos, cap, ctx->err);
 }
 
+int jsgpu_find_markers(jsgpu_ctx* ctx, const uint8_t* data, uint64_t n, const jsgpu_overlay* overlays, uint32_t noverlays,
+                       uint32_t* soi_pos, uint64_t soi_cap, uint64_t* nsoi, uint32_t* term_pos, uint64_t term_cap, uint64_t* nterm)
+{
+    if (!ctx) return JSGPU_EINVAL;
+    if (!nsoi || !nterm || (n && !data) || (noverlays && !overlays) || (soi_cap && !soi_pos) || (term_cap && !term_pos))
+        return fail(ctx, JSGPU_EINVAL, "jsgpu_find_markers: bad arguments");
+    for (uint32_t k = 0; k < noverlays; k++)
+        if (overlays[k].len && !overlays[k].data) return fail(ctx, JSGPU_EINVAL, "jsgpu_find_markers: overlay %u has no data", k);
+    if (n >> 32)
+        return fail(ctx, JSGPU_EINVAL, "jsgpu_find_markers: %llu bytes: files of 2^32 bytes or more do not fit 32-bit offsets",
+                    (unsigned long long)n);
+    return js_find_markers_run(&ctx->search, ctx->device, ctx->sm_count, data, n, overlays, noverlays, soi_pos, soi_cap, nsoi,
+                               term_pos, term_cap, nterm, ctx->err);
+}
+
 void* jsgpu_host_alloc(uint64_t bytes) { void* p = nullptr; if (cudaMallocHost(&p, bytes) != cudaSuccess) return nullptr; return p; }
 void  jsgpu_host_free(void* p) { if (p) cudaFreeHost(p); }
 

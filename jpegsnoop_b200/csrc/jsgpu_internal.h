@@ -231,6 +231,9 @@ int  js_find_run(JsSearch** s, int device, int sm_count, const uint8_t* data, ui
                  uint32_t len, int forward, const jsgpu_overlay* ovl, uint32_t novl, int* found, uint64_t* found_pos, std::string& err);
 int  js_find_all_run(JsSearch** s, int device, int sm_count, const uint8_t* data, uint64_t n, uint32_t value, uint32_t len,
                      uint64_t* count, uint32_t* pos, uint64_t cap, std::string& err);
+int  js_find_markers_run(JsSearch** s, int device, int sm_count, const uint8_t* data, uint64_t n, const jsgpu_overlay* ovl,
+                         uint32_t novl, uint32_t* soi_pos, uint64_t soi_cap, uint64_t* nsoi, uint32_t* term_pos, uint64_t term_cap,
+                         uint64_t* nterm, std::string& err);
 void js_search_free(JsSearch* s);
 #define JSGPU_CK_WORDS_INTERNAL 12   // == JSGPU_CK_WORDS (include/jsgpu.h)
 int js_launch_checksums(const DevBatch& b, unsigned long long* ck, cudaStream_t s);

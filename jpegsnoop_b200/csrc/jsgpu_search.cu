@@ -18,8 +18,8 @@
 //                          anything, in file order, into a compact per-chunk list the host copies into place.
 // Device memory is two chunk buffers, the per-tile summaries and one chunk's emitted positions, whatever the file size.
 // The search has its own streams and buffers: a batch resident on the same context is not touched.
-// The first-match value search of Img Search Fwd / Rev (jsgpu_find_value) and the every-match value search (jsgpu_find_all),
-// both at the end of the file, share them.
+// The first-match value search of Img Search Fwd / Rev (jsgpu_find_value), the every-match value search (jsgpu_find_all)
+// and the extract walk's marker search (jsgpu_find_markers), all at the end of the file, share them.
 #include "jsgpu_internal.h"
 #include <cstdlib>
 #include <cstring>
@@ -621,47 +621,85 @@ int js_find_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, ui
     return JSGPU_OK;
 }
 
-// ---- every match of a value (jsgpu_find_all, include/jsgpu.h) ----------------------------------------------------------
+// ---- every match of a value (jsgpu_find_all) and the extract walk's markers (jsgpu_find_markers), include/jsgpu.h -------
 // Each chunk is uploaded once and stays resident while three kernels run on it: k_find_all<false> counts the matches of
 // each CTA's run of consecutive tiles, k_find_all_scan turns the counts into output indices from the running total kept on
 // the device, and k_find_all<true> writes the positions in file order.  CTA b owns tiles [b * per, (b + 1) * per).
-template <bool EMIT>
+// A search lists one or two match sets over the same chunk: a value (fv_match16) or the scan terminators (fv_term16).
+
+// The PASS-1 scan terminators among positions p0 .. p0 + 15 (p0 a multiple of 16): p with buf[p] == FF and buf[p + 1]
+// neither 00 nor D0..D7 (JfifDecode.cpp:5194-5265).  buf holds npos + 1 bytes and is readable as fv_match16's.
+__device__ __forceinline__ uint32_t fv_term16(const uint8_t* __restrict__ buf, uint32_t p0, uint32_t npos)
+{
+    uint32_t m = 0;
+    if (p0 < npos) {
+        const uint4 a = *(const uint4*)(buf + p0);
+        const uint32_t w[5] = {a.x, a.y, a.z, a.w, *(const uint32_t*)(buf + p0 + 16)};
+#pragma unroll
+        for (int k = 0; k < 16; k++) {
+            const uint32_t v = (k % 4) ? __funnelshift_r(w[k / 4], w[k / 4 + 1], 8 * (k % 4)) : w[k / 4];
+            const uint32_t b1 = (v >> 8) & 0xFFu;
+            if ((v & 0xFFu) == 0xFFu && b1 != 0u && (b1 & 0xF8u) != 0xD0u) m |= 1u << k;
+        }
+        if (npos - p0 < 16) m &= (1u << (npos - p0)) - 1u;
+    }
+    return m;
+}
+
+// One match set of a chunk: the value pat / mask at positions 0 .. npos - 1, or the terminators there when `term`; the
+// positions go to out, at most cap of them in all.
+struct FaSet { uint32_t npos, pat, mask, term; uint32_t* out; uint64_t cap; };
+struct FaSets { FaSet s[2]; };
+
+__device__ __forceinline__ uint32_t fa_match16(const uint8_t* __restrict__ buf, uint32_t p0, const FaSet& f)
+{
+    return f.term ? fv_term16(buf, p0, f.npos) : fv_match16(buf, p0, f.npos, f.pat, f.mask);
+}
+
+template <bool EMIT, int NSET>
 __global__ void __launch_bounds__(SR_THREADS)
-k_find_all(const uint8_t* __restrict__ buf, uint32_t npos, uint32_t pat, uint32_t mask, uint32_t per, uint32_t chunk_pos,
-           uint32_t* __restrict__ cta /*[2][gridDim.x]: counts, then first output index*/, uint32_t* __restrict__ out, uint64_t cap)
+k_find_all(const uint8_t* __restrict__ buf, uint32_t npos, FaSets sets, uint32_t per, uint32_t chunk_pos,
+           uint32_t* __restrict__ cta /*[NSET][2][gridDim.x]: counts, then first output index*/)
 {
     __shared__ uint32_t s_w[SR_THREADS / 32 + 1];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t ntiles = (npos + SR_TILE - 1) / SR_TILE;
     const uint32_t t0 = blockIdx.x * per, t1 = min(ntiles, t0 + per);
-    if (!EMIT) {
-        uint32_t c = 0;
-        for (uint32_t t = t0; t < t1; t++) c += __popc(fv_match16(buf, t * SR_TILE + 16 * tid, npos, pat, mask));
-        c = __reduce_add_sync(0xffffffffu, c);
-        if (lane == 0) s_w[warp] = c;
-        __syncthreads();
-        if (tid == 0) {
-            uint32_t sum = 0;
-            for (int k = 0; k < SR_THREADS / 32; k++) sum += s_w[k];
-            cta[blockIdx.x] = sum;
+#pragma unroll
+    for (int k = 0; k < NSET; k++) {
+        const FaSet& f = sets.s[k];
+        uint32_t* const ck = cta + 2 * gridDim.x * k;
+        if (!EMIT) {
+            uint32_t c = 0;
+            for (uint32_t t = t0; t < t1; t++) c += __popc(fa_match16(buf, t * SR_TILE + 16 * tid, f));
+            c = __reduce_add_sync(0xffffffffu, c);
+            if (lane == 0) s_w[warp] = c;
+            __syncthreads();
+            if (tid == 0) {
+                uint32_t sum = 0;
+                for (int w = 0; w < SR_THREADS / 32; w++) sum += s_w[w];
+                ck[blockIdx.x] = sum;
+            }
+            __syncthreads();
+            continue;
         }
-        return;
-    }
-    uint32_t j = cta[gridDim.x + blockIdx.x];                // this CTA's first output index
-    if (cta[blockIdx.x] == 0 || j >= cap) return;
-    for (uint32_t t = t0; t < t1 && j < cap; t++) {
-        uint32_t m = fv_match16(buf, t * SR_TILE + 16 * tid, npos, pat, mask);
-        uint64_t o = block_scan<SR_THREADS>((uint32_t)__popc(m), 0u, sr_add, j, s_w);   // advances j past the tile
-        const uint32_t p = chunk_pos + t * SR_TILE + 16 * tid;
-        while (m && o < cap) { out[o++] = p + (uint32_t)__ffs((int)m) - 1; m &= m - 1; }
+        uint32_t j = ck[gridDim.x + blockIdx.x];             // this CTA's first output index
+        if (ck[blockIdx.x] == 0 || j >= f.cap) continue;
+        for (uint32_t t = t0; t < t1 && j < f.cap; t++) {
+            uint32_t m = fa_match16(buf, t * SR_TILE + 16 * tid, f);
+            uint64_t o = block_scan<SR_THREADS>((uint32_t)__popc(m), 0u, sr_add, j, s_w);   // advances j past the tile
+            const uint32_t p = chunk_pos + t * SR_TILE + 16 * tid;
+            while (m && o < f.cap) { f.out[o++] = p + (uint32_t)__ffs((int)m) - 1; m &= m - 1; }
+        }
     }
 }
 
-// One CTA: the first output index of every CTA of the chunk, from the running total, which it then advances.
+// CTA k: the first output index of every CTA of the chunk in set k, from set k's running total, which it then advances.
 __global__ void __launch_bounds__(1024)
 k_find_all_scan(uint32_t* __restrict__ cta, uint32_t ncta, uint32_t* __restrict__ total)
 {
     __shared__ uint32_t s_w[33];
+    cta += 2 * ncta * blockIdx.x; total += blockIdx.x;
     uint32_t run = *total;
     for (uint32_t b0 = 0; b0 < ncta; b0 += 1024) {
         const uint32_t b = b0 + threadIdx.x;
@@ -671,48 +709,95 @@ k_find_all_scan(uint32_t* __restrict__ cta, uint32_t ncta, uint32_t* __restrict_
     if (threadIdx.x == 0) *total = run;
 }
 
+// One streaming pass of NSET match sets over positions 0 .. npos - 1 of the file, chunks carrying `halo` bytes.  set(k, plo,
+// cnpos) gives set k's FaSet for the chunk of cnpos positions from plo (npos, pat, mask, term); counts[k] receive complete
+// counts and pos[k] at most caps[k] positions.
+template <int NSET, typename SetOf>
+static int fa_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, uint64_t n, uint64_t npos, uint32_t halo,
+                  const jsgpu_overlay* ovl, uint32_t novl, SetOf set, uint64_t* counts, uint32_t* const* pos, const uint64_t* caps,
+                  std::string& err)
+{
+    for (int k = 0; k < NSET; k++) counts[k] = 0;
+    if (!npos) return JSGPU_OK;
+    const SrChunks ch(n, 0, npos, halo, false);
+    SR_TRY(sr_open(ps, device, ch, err));
+    JsSearch* s = *ps;
+    int occ = 0;
+    SR_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_find_all<true, NSET>, SR_THREADS, 0));
+    const uint32_t grid_max = (uint32_t)(std::max(occ, 1) * sm_count);
+    for (int i = 0; i < 2; i++) SR_CK(s->cta[i].reserve(2 * NSET * (size_t)grid_max * 4));
+    uint64_t keep[NSET], off[NSET], all = 0;                  // positions each device list can hold, and where it starts
+    for (int k = 0; k < NSET; k++) { keep[k] = std::min<uint64_t>(caps[k], ch.npos); off[k] = all; all += keep[k]; }
+    if (all) SR_CK(s->out.reserve(all * 4));
+    SR_CK(s->total.reserve(4 * NSET));
+    uint32_t* const total = s->total.as<uint32_t>();
+    SR_CK(cudaMemsetAsync(total, 0, 4 * NSET, s->st[0]));
+    SR_CK(cudaEventRecord(s->scanned[1], s->st[0]));                      // chunk 0's scan follows the reset
+
+    bool emit = false;
+    for (int k = 0; k < NSET; k++) emit |= keep[k] != 0;
+    for (uint64_t c = 0; c < ch.count; c++) {
+        const int sl = (int)(c & 1);
+        const uint32_t cnpos = ch.positions(c), plo = (uint32_t)ch.first(c);
+        SR_TRY(sr_stage(s, ch, c, data, ovl, novl, err));
+        SR_TRY(sr_send(s, ch, c, err));
+        const uint8_t* const buf = s->buf[sl].as<uint8_t>();
+        uint32_t* const cta = s->cta[sl].as<uint32_t>();
+        FaSets sets = {};
+        for (int k = 0; k < NSET; k++) {
+            sets.s[k] = set(k, plo, cnpos);
+            sets.s[k].out = s->out.as<uint32_t>() + off[k];
+            sets.s[k].cap = keep[k];
+        }
+        const uint32_t ntiles = (cnpos + SR_TILE - 1) / SR_TILE;
+        const uint32_t grid = std::max(1u, std::min(grid_max, ntiles)), per = (ntiles + grid - 1) / grid;
+        k_find_all<false, NSET><<<grid, SR_THREADS, 0, s->st[sl]>>>(buf, cnpos, sets, per, plo, cta);
+        SR_CK(cudaStreamWaitEvent(s->st[sl], s->scanned[sl ^ 1], 0));  // the previous chunk has advanced the totals
+        k_find_all_scan<<<NSET, 1024, 0, s->st[sl]>>>(cta, grid, total);
+        SR_CK(cudaEventRecord(s->scanned[sl], s->st[sl]));
+        if (emit) k_find_all<true, NSET><<<grid, SR_THREADS, 0, s->st[sl]>>>(buf, cnpos, sets, per, plo, cta);
+        SR_CK(cudaGetLastError());
+    }
+    SR_CK(cudaStreamSynchronize(s->st[0])); SR_CK(cudaStreamSynchronize(s->st[1]));
+    uint32_t tot[NSET];
+    SR_CK(cudaMemcpy(tot, total, 4 * NSET, cudaMemcpyDeviceToHost));
+    for (int k = 0; k < NSET; k++) {
+        counts[k] = tot[k];
+        const uint64_t got = std::min<uint64_t>(tot[k], keep[k]);
+        if (got) SR_CK(cudaMemcpy(pos[k], s->out.as<uint32_t>() + off[k], got * 4, cudaMemcpyDeviceToHost));
+    }
+    return JSGPU_OK;
+}
+
 int js_find_all_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, uint64_t n, uint32_t value, uint32_t len,
                     uint64_t* count, uint32_t* pos, uint64_t cap, std::string& err)
 {
     *count = 0;
     const uint32_t mask = len == 4 ? 0xFFFFFFFFu : (1u << (8 * len)) - 1u;
     if (n < len || (value & ~mask)) return JSGPU_OK;         // no position, or a value wider than len bytes
-    const SrChunks ch(n, 0, n - len + 1, len - 1, false);
-    SR_TRY(sr_open(ps, device, ch, err));
-    JsSearch* s = *ps;
-    int occ = 0;
-    SR_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_find_all<true>, SR_THREADS, 0));
-    const uint32_t grid_max = (uint32_t)(std::max(occ, 1) * sm_count);
-    for (int i = 0; i < 2; i++) SR_CK(s->cta[i].reserve(2 * (size_t)grid_max * 4));
-    const uint64_t keep = std::min<uint64_t>(cap, ch.npos);   // positions the device list can hold
-    if (keep) SR_CK(s->out.reserve(keep * 4));
-    SR_CK(s->total.reserve(4));
     const uint32_t pat = __builtin_bswap32(value) >> (32 - 8 * len);      // the bytes in file order, little-endian
-    uint32_t* const total = s->total.as<uint32_t>();
-    SR_CK(cudaMemsetAsync(total, 0, 4, s->st[0]));
-    SR_CK(cudaEventRecord(s->scanned[1], s->st[0]));                      // chunk 0's scan follows the reset
+    auto set = [&](int, uint32_t, uint32_t cnpos) { return FaSet{cnpos, pat, mask, 0u, nullptr, 0}; };
+    return fa_run<1>(ps, device, sm_count, data, n, n - len + 1, len - 1, nullptr, 0, set, count, &pos, &cap, err);
+}
 
-    for (uint64_t c = 0; c < ch.count; c++) {
-        const int sl = (int)(c & 1);
-        const uint32_t npos = ch.positions(c), plo = (uint32_t)ch.first(c);
-        SR_TRY(sr_stage(s, ch, c, data, nullptr, 0, err));
-        SR_TRY(sr_send(s, ch, c, err));
-        const uint8_t* const buf = s->buf[sl].as<uint8_t>();
-        uint32_t* const cta = s->cta[sl].as<uint32_t>();
-        const uint32_t ntiles = (npos + SR_TILE - 1) / SR_TILE;
-        const uint32_t grid = std::max(1u, std::min(grid_max, ntiles)), per = (ntiles + grid - 1) / grid;
-        k_find_all<false><<<grid, SR_THREADS, 0, s->st[sl]>>>(buf, npos, pat, mask, per, plo, cta, nullptr, 0);
-        SR_CK(cudaStreamWaitEvent(s->st[sl], s->scanned[sl ^ 1], 0));  // the previous chunk has advanced the total
-        k_find_all_scan<<<1, 1024, 0, s->st[sl]>>>(cta, grid, total);
-        SR_CK(cudaEventRecord(s->scanned[sl], s->st[sl]));
-        if (keep) k_find_all<true><<<grid, SR_THREADS, 0, s->st[sl]>>>(buf, npos, pat, mask, per, plo, cta, s->out.as<uint32_t>(), keep);
-        SR_CK(cudaGetLastError());
-    }
-    SR_CK(cudaStreamSynchronize(s->st[0])); SR_CK(cudaStreamSynchronize(s->st[1]));
-    uint32_t tot = 0;
-    SR_CK(cudaMemcpy(&tot, total, 4, cudaMemcpyDeviceToHost));
-    *count = tot;
-    const uint64_t got = std::min<uint64_t>(tot, keep);
-    if (got) SR_CK(cudaMemcpy(pos, s->out.p, got * 4, cudaMemcpyDeviceToHost));
+// Set 0: FF D8 FF at 0 .. n - 3; set 1: the terminators at 0 .. n - 2 (an FF in the last byte is followed by 0, the byte
+// Buf() reads past the end of the file, so it ends nothing).  Chunks cover the terminator positions with 2 halo bytes.
+int js_find_markers_run(JsSearch** ps, int device, int sm_count, const uint8_t* data, uint64_t n, const jsgpu_overlay* ovl,
+                        uint32_t novl, uint32_t* soi_pos, uint64_t soi_cap, uint64_t* nsoi, uint32_t* term_pos, uint64_t term_cap,
+                        uint64_t* nterm, std::string& err)
+{
+    *nsoi = *nterm = 0;
+    if (n < 2) return JSGPU_OK;
+    const uint64_t nsoi_pos = n >= 3 ? n - 2 : 0;
+    auto set = [&](int k, uint32_t plo, uint32_t cnpos) {
+        if (k == 1) return FaSet{cnpos, 0u, 0u, 1u, nullptr, 0};
+        const uint32_t np = plo < nsoi_pos ? (uint32_t)std::min<uint64_t>(cnpos, nsoi_pos - plo) : 0u;
+        return FaSet{np, 0xFFD8FFu, 0xFFFFFFu, 0u, nullptr, 0};           // FF D8 FF read little-endian is FF D8 FF
+    };
+    uint64_t counts[2];
+    uint32_t* const pos[2] = {soi_pos, term_pos};
+    const uint64_t caps[2] = {soi_cap, term_cap};
+    SR_TRY(fa_run<2>(ps, device, sm_count, data, n, n - 1, 2, ovl, novl, set, counts, pos, caps, err));
+    *nsoi = counts[0]; *nterm = counts[1];
     return JSGPU_OK;
 }

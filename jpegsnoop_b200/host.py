@@ -217,6 +217,35 @@ class CimgDecode:
             raise JsgpuError(f"jsimg_buf_search failed ({r}): {self.log_lines(3)}")
         return bool(r), p.value
 
+    def export_jpeg(self, data, out_path, offset=0, overlay=False, force_soi=False, force_eoi=False, ignore_eoi=False,
+                    dht_avi_insert=False, overlays=(), src_name="input.bin"):
+        """Tools -> Extract embedded JPEG (JPEGsnoopCore.cpp:913-961): the frame at `offset` of `data` (bytes or a uint8 array)
+        walked to its EOI, its scans skipped on the GPU, written to out_path as ExportJpegPrepare / ExportJpegDo write it.
+        `overlays` [(start, bytes), ...] are installed for the walk; `overlay` copies the bytes through them too.  src_name is
+        the source file's name (the log names it, and an out_path equal to it is refused).  Returns (written, the export's
+        log lines); raises JsgpuError when the GPU search fails."""
+        return self._export(data, overlays, lambda f: self.L.jsimg_export_jpeg(self.h, offset, str(src_name).encode(),
+                                                                                str(out_path).encode(), f),
+                            overlay, force_soi, force_eoi, ignore_eoi, dht_avi_insert)
+
+    def _export(self, data, overlays, run, *opts):
+        self._file = _u8(data)
+        self.L.jsimg_set_file(self.h, self._file.ctypes.data, self._file.size)
+        self.L.jsimg_overlay_remove_all(self.h)
+        keep = [np.frombuffer(bytes(b), np.uint8) for _, b in overlays]
+        for (o, _), a in zip(overlays, keep):
+            self.L.jsimg_overlay_install(self.h, int(o), a.ctypes.data, a.size)
+        self.L.jsimg_log_clear(self.h)
+        flags = sum(1 << k for k, v in enumerate(opts) if v)
+        try:
+            r = run(flags)
+        finally:
+            self.L.jsimg_overlay_remove_all(self.h)
+        lines = self.log_lines()
+        if r < 0 and not (r == -2 and lines and lines[-1].startswith("ERROR: Invalid filename")):
+            raise JsgpuError(f"export failed ({r}): {lines[-3:]}")
+        return r, lines
+
     def _img_search(self, start, forward, quiet):
         found, pos, decoded = C.c_int(0), C.c_uint64(0), C.c_int(0)
         self.L.jsimg_log_clear(self.h)
@@ -317,12 +346,15 @@ class BatchDecoder:
                                    scan_err_max=20)
         self._ck(self.L.jsgpu_set_options(self.ctx, C.byref(self.opt)))
         self.n = 0; self.layout = None; self.descs = None; self.bitstream = None; self.nsof_pixels = 0
+        self._jsimg = None                    # extract_all's host walker and log, made on first use
 
     def _ck(self, r):
         if r != 0:
             raise JsgpuError(f"{self.L.jsgpu_strerror(r).decode()}: {self.L.jsgpu_last_error(self.ctx).decode()}")
 
     def close(self):
+        if self._jsimg is not None:
+            self._jsimg.close(); self._jsimg = None
         if self.ctx:
             self.L.jsgpu_free(self.ctx); self.ctx = None
 
@@ -439,6 +471,35 @@ class BatchDecoder:
             want = count.value; pos = np.zeros(want, np.uint32)
             self._ck(self.L.jsgpu_find_all(self.ctx, buf.ctypes.data, buf.size, value, length, C.byref(count), pos.ctypes.data, want))
         return int(count.value), pos[:min(int(count.value), int(want))]
+
+    def extract_all(self, data, out_name, overlay=False, force_soi=False, force_eoi=False, ignore_eoi=False,
+                    dht_avi_insert=False, overlays=(), src_name="input.bin"):
+        """Extract All (JPEGsnoopCore.cpp:963-1088; the command line's -ext_all): every frame from offset 0 and from each FF D8 FF
+        after the last start, written to root.000001.jpg, root.000002.jpg, ... (root: out_name up to its last '.').  The search
+        runs on this context; a resident batch is left untouched.  Options as CimgDecode.export_jpeg.  Returns
+        ([(offset, path or None)] per frame analysed, the export log lines); with no '.' in out_name, ([], the error line)."""
+        if self._jsimg is None:
+            self._jsimg = CimgDecode(device=self.device)
+        d = self._jsimg
+        want = _u8(data).size // 4096 + 1024          # frames analysed: one more than the FF D8 FF after offset 0
+        offs = np.zeros(want, np.uint64); nums = np.zeros(want, np.uint32)
+
+        def run(flags):
+            nonlocal offs, nums
+            a = (C.c_char_p(str(src_name).encode()), C.c_char_p(str(out_name).encode()), flags)
+            k = self.L.jsimg_extract_all(d.h, self.ctx, *a, offs.ctypes.data, nums.ctypes.data, offs.size)
+            if k > offs.size:                         # more frames than the guess holds: run again with room for all
+                d.L.jsimg_log_clear(d.h)
+                offs = np.zeros(k, np.uint64); nums = np.zeros(k, np.uint32)
+                k = self.L.jsimg_extract_all(d.h, self.ctx, *a, offs.ctypes.data, nums.ctypes.data, k)
+            offs, nums = offs[:max(k, 0)], nums[:max(k, 0)]
+            return k
+
+        r, lines = d._export(data, overlays, run, overlay, force_soi, force_eoi, ignore_eoi, dht_avi_insert)
+        if r < 0:
+            return [], lines
+        root = str(out_name)[:str(out_name).rfind(".")]
+        return [(int(o), f"{root}.{int(m):06d}.jpg" if m else None) for o, m in zip(offs, nums)], lines
 
     def decode_all(self, data, redo_budget=1 << 30):
         """Every JPEG in `data` in one batch: the SOI candidates of find_all(), each walked from its offset, each walked image
