@@ -14,6 +14,7 @@
 //                   previous interval left the reader, the map entry of that MCU, ImgDecode.cpp:1644-1680, 3229).
 // Damaged images take the serial walk instead (jsgpu_exact.cu): resynchronisation and lazy restarts are not interval-local.
 #include "jsgpu_detail.cuh"
+#include "jsgpu_scan.cuh"
 #include <climits>
 
 #define DT_THREADS 128
@@ -136,34 +137,18 @@ __global__ void __launch_bounds__(DT_THREADS) k_detail_count(DevBatch b, JsDetai
 
 __global__ void __launch_bounds__(1024) k_detail_scan(DevBatch b, JsDetailRange r, uint32_t* cnt, const uint32_t* lastp, uint32_t* hdr, JsErrCfg cfg)
 {
-    __shared__ uint32_t s_warp[32];
-    __shared__ uint32_t s_carry;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) s_carry = 0;
-    __syncthreads();
+    __shared__ uint32_t s_warp[33];
+    const uint32_t tid = threadIdx.x;
+    uint32_t total = 0;
     for (uint32_t base = 0; base < r.n; base += 1024) {
-        const uint32_t i = base + tid, v = (i < r.n) ? cnt[i] : 0u;
-        uint32_t x = v;
-        #pragma unroll
-        for (uint32_t o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-        if (lane == 31) s_warp[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            uint32_t w = s_warp[lane];
-            #pragma unroll
-            for (uint32_t o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-            s_warp[lane] = w;
-        }
-        __syncthreads();
-        const uint32_t excl = s_carry + (warp ? s_warp[warp - 1] : 0u) + x - v;
-        if (i < r.n) cnt[i] = excl;
-        __syncthreads();
-        if (tid == 1023) s_carry = excl + v;
-        __syncthreads();
+        uint32_t* const c = cnt + base + tid;
+        const bool in = base + tid < r.n;
+        const uint32_t excl = js_block_scan<1024>(in ? *c : 0u, 0u, js_add, total, s_warp);
+        if (in) *c = excl;
     }
     if (tid != 0) return;
     const DevImage& im = b.img[r.image];
-    hdr[0] = s_carry; hdr[1] = r.nprint * im.bpm;
+    hdr[0] = total; hdr[1] = r.nprint * im.bpm;
     // the end-of-scan marker note (BuffAddByte, ImgDecode.cpp:1527-1543) when the walk's last top-up reaches it and the cap still
     // allows a line, plus the cap line when this one reaches it (:1100-1110); the fields the walk sets for a healthy image, the
     // others as they were
@@ -173,19 +158,10 @@ __global__ void __launch_bounds__(1024) k_detail_scan(DevBatch b, JsDetailRange 
     if (r.n) met = (r.first + r.n - 1) / im.ri + 1 == im.nseg && (long long)lastp[r.n - 1] >= T;
     else met = im.nseg == 1 && 0 >= T;                           // nothing decoded: the first top-up only
     JsExResult* res = b.ex_res + r.image;
-    res->nerr_lines = 0; res->nevents = 0; res->scan_bad = 0; res->restart_read = 0; res->done = 0;
-    res->warn_num = cfg.warn_start;
-    if (met && cfg.warn_start < cfg.err_max) {
-        JsExEvent& e = res->ev[0];
-        e.code = JS_EX_MARKER_NOTE; e.a = marker; e.b = im.file_pos + b.scan_end[r.image]; e.c = e.d = e.e = 0; e.pad0 = e.pad1 = 0;
-        res->nevents = 1; res->nerr_lines = (marker != 0xD9) ? 1u : 0u;
-        res->warn_num = cfg.warn_start + 1;
-        if (res->warn_num >= cfg.err_max) {
-            JsExEvent& c = res->ev[1];
-            c.code = JS_EX_CAP; c.a = cfg.err_max; c.b = c.c = c.d = c.e = 0; c.pad0 = c.pad1 = 0;
-            res->nevents = 2; res->nerr_lines++;
-        }
-    }
+    js_ex_reset(res);
+    uint32_t warn = cfg.warn_start;
+    if (met) js_ex_warn(res, res->ev, JS_EX_MAX_EVENTS, cfg.err_max, warn, JS_EX_MARKER_NOTE, marker != 0xD9, marker, im.file_pos + b.scan_end[r.image]);
+    res->warn_num = warn;
 }
 
 __global__ void __launch_bounds__(DT_THREADS) k_detail_emit(DevBatch b, JsDetailRange r, const uint32_t* off, const uint32_t* lastp, JsDetailOut out)

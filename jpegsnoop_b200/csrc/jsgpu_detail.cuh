@@ -1,7 +1,7 @@
 // jsgpu_detail.cuh — what the serial reference-semantics walk (jsgpu_exact.cu) and the parallel "Detailed Decode" kernels
 // (jsgpu_detail.cu) share: the file position of an unstuffed byte (also the MCU file map's, jsgpu_kernels.cu), the code search
-// and value decode of ReadScanVal, the dequantising store of DecodeIdctSet, and the encoding of DecodeScanCompPrint's report
-// lines as jsgpu_detail_events.
+// and value decode of ReadScanVal, the dequantising store of DecodeIdctSet, the encoding of DecodeScanCompPrint's report
+// lines as jsgpu_detail_events, and the scan-error report's events and cap rule.
 #pragma once
 #include "jsgpu_internal.h"
 
@@ -101,4 +101,27 @@ __device__ __forceinline__ void js_detail_vlc(jsgpu_detail_event& ev, uint32_t s
                                               uint32_t coef_start, uint32_t coef_end, uint32_t bits, uint32_t special)
 {
     js_detail_put(ev, JSGPU_DT_VLC, seq, pos, align, zrl, (uint32_t)(int)val, coef_start | (coef_end << 8) | (bits << 16), special);
+}
+
+// The scan-error report (jsgpu_scan_errors): counts back to a scan's start (warn_num and the end position are set by the caller).
+__device__ __forceinline__ void js_ex_reset(JsExResult* res)
+{
+    res->nerr_lines = 0; res->nevents = 0; res->scan_bad = 0; res->restart_read = 0; res->done = 0;
+}
+// One error event making `lines` error lines; ev[] (cap entries) keeps the first ones, the counts go on.
+__device__ __forceinline__ void js_ex_event(JsExResult* res, JsExEvent* ev, uint32_t cap, uint32_t code, uint32_t lines,
+                                            uint32_t a = 0, uint32_t b = 0, uint32_t c = 0, uint32_t d = 0, uint32_t e = 0)
+{
+    res->nerr_lines += lines;
+    if (res->nevents < cap) ev[res->nevents] = JsExEvent{code, a, b, c, d, e, 0, 0};
+    res->nevents++;
+}
+// The "first nErrMaxDecodeScan instances" rule (ImgDecode.cpp:1100-1110 and its copies): the event only while fewer than
+// err_max have been counted in `warn` (m_nWarnBadScanNum), and the cap line after the one that reaches err_max.
+__device__ __forceinline__ void js_ex_warn(JsExResult* res, JsExEvent* ev, uint32_t cap, uint32_t err_max, uint32_t& warn, uint32_t code,
+                                           uint32_t lines, uint32_t a = 0, uint32_t b = 0, uint32_t c = 0, uint32_t d = 0, uint32_t e = 0)
+{
+    if (warn >= err_max) return;
+    js_ex_event(res, ev, cap, code, lines, a, b, c, d, e);
+    if (++warn >= err_max) js_ex_event(res, ev, cap, JS_EX_CAP, 1, err_max);
 }

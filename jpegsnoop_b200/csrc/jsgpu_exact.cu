@@ -50,19 +50,11 @@ __device__ __forceinline__ void ex_detail(Ex& x, uint32_t kind, uint32_t a = 0, 
 
 __device__ __forceinline__ void ex_event(Ex& x, uint32_t code, uint32_t lines, uint32_t a = 0, uint32_t b = 0, uint32_t c = 0, uint32_t d = 0, uint32_t e = 0)
 {
-    JsExResult* r = x.res;
-    r->nerr_lines += lines;
-    if (r->nevents < x.ev_cap) { JsExEvent& ev = x.ev[r->nevents]; ev.code = code; ev.a = a; ev.b = b; ev.c = c; ev.d = d; ev.e = e; ev.pad0 = ev.pad1 = 0; }
-    r->nevents++;
+    js_ex_event(x.res, x.ev, x.ev_cap, code, lines, a, b, c, d, e);
 }
-// the "first nErrMaxDecodeScan instances" pattern (ImgDecode.cpp:1100-1110 and its copies)
 __device__ __forceinline__ void ex_warn(Ex& x, uint32_t code, uint32_t lines, uint32_t a = 0, uint32_t b = 0, uint32_t c = 0, uint32_t d = 0, uint32_t e = 0)
 {
-    if (x.warn_bad_num < x.err_max) {
-        ex_event(x, code, lines, a, b, c, d, e);
-        x.warn_bad_num++;
-        if (x.warn_bad_num >= x.err_max) ex_event(x, JS_EX_CAP, 1, x.err_max);
-    }
+    js_ex_warn(x.res, x.ev, x.ev_cap, x.err_max, x.warn_bad_num, code, lines, a, b, c, d, e);
 }
 __device__ __forceinline__ uint32_t ex_fbuf(const Ex& x, uint32_t off) { return (off < x.n) ? (uint32_t)__ldg(x.data + off) : 0u; }   // WindowBuf.cpp:639-713: bytes past EOF read as 0
 
@@ -106,11 +98,7 @@ __device__ __noinline__ void ex_buff_add_byte(Ex& x)
     if (b0 == 0xFF && b1 == 0x00)      { ex_scanbuf_add(x, b0, x.file_pos + x.ptr, EX_SCANBUF_OK); x.ptr += 2; }
     else if (b0 == 0xFF && b1 == 0xFF) { ex_scanbuf_add(x, b0, x.file_pos + x.ptr, EX_SCANBUF_OK); x.ptr += 1; }
     else if (b0 == 0xFF && marker != 0) {
-        if (x.warn_bad_num < x.err_max) {
-            ex_event(x, JS_EX_MARKER_NOTE, (marker != 0xD9) ? 1u : 0u, marker, x.file_pos + x.ptr);        // one normal line; an error line too unless it is EOI
-            x.warn_bad_num++;
-            if (x.warn_bad_num >= x.err_max) ex_event(x, JS_EX_CAP, 1, x.err_max);
-        }
+        ex_warn(x, JS_EX_MARKER_NOTE, marker != 0xD9, marker, x.file_pos + x.ptr);        // one normal line; an error line too unless it is EOI
         ex_scanbuf_add(x, b0, x.file_pos + x.ptr, EX_SCANBUF_BADMARK); x.ptr += 1;
     } else { ex_scanbuf_add(x, b0, x.file_pos + x.ptr, EX_SCANBUF_OK); x.ptr += 1; }
 }
@@ -261,7 +249,7 @@ __device__ __forceinline__ void ex_walk(const DevBatch& b, uint32_t ii, const Js
     x.ts = b.tables + im.table_set;
     x.res = res; x.histo = wr ? b.histo + (size_t)ii * JSGPU_HISTO_WORDS : scratch_histo;
     x.ev = evonly ? ev_all : res->ev; x.ev_cap = evonly ? ev_cap : JS_EX_MAX_EVENTS;
-    x.res->nerr_lines = 0; x.res->nevents = 0; x.res->scan_bad = 0; x.res->restart_read = 0; x.res->done = 0;
+    js_ex_reset(x.res);
     x.err_max = cfg.err_max; x.warn_bad_num = cfg.warn_start; x.errs_off = cfg.disable != 0;
     x.precision = im.precision; x.decode_ac = b.decode_ac != 0;
     x.rst_interval = im.restart_en ? im.ri : 0;                 // m_nRestartInterval (0 when DRI is off: never looked at then)

@@ -17,6 +17,7 @@
 // holds the running DC predictor sum (m_nDcLum += m_anDctBlock[0], :3280).
 #include "jsgpu_internal.h"
 #include "jsgpu_phuff_core.cuh"
+#include "jsgpu_scan.cuh"
 #include <algorithm>
 #include <cstdlib>
 
@@ -353,11 +354,9 @@ __global__ void __launch_bounds__(128) k_unstuff_scan(DevBatch b)
             const size_t c0 = im.cs_first + ul_base(s0, k);
             uint32_t run = 0;
             for (uint32_t c = 0; c < nch; c += 32) {
-                const uint32_t v = (c + lane < nch) ? b.cs_cnt[c0 + c + lane] : 0u;
-                uint32_t inc = v;
-                #pragma unroll
-                for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(FULL, inc, d); if (lane >= (uint32_t)d) inc += y; }
-                if (c + lane < nch) b.cs_off[c0 + c + lane] = run + inc - v;
+                uint32_t inc;
+                const uint32_t ex = js_warp_scan((c + lane < nch) ? b.cs_cnt[c0 + c + lane] : 0u, 0u, js_add, inc);
+                if (c + lane < nch) b.cs_off[c0 + c + lane] = run + ex;
                 run += __shfl_sync(FULL, inc, 31);
             }
             if (lane == 0) {

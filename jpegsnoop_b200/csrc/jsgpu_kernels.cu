@@ -16,6 +16,7 @@
 #include "jsgpu_internal.h"
 #include "jsgpu_ycc.cuh"
 #include "jsgpu_detail.cuh"     // js_raw_of_unstuffed
+#include "jsgpu_scan.cuh"
 #include <cstdio>
 #include <cstdlib>
 #include <algorithm>
@@ -77,7 +78,7 @@ __global__ void __launch_bounds__(MS_THREADS) k_marker_scan(DevBatch b)
     __shared__ uint32_t s_term;
     const uint8_t* p = b.bits + im.scan_off;
     const uint64_t n = im.scan_len;
-    const uint32_t t = threadIdx.x, lane = t & 31, wid = t >> 5;
+    const uint32_t t = threadIdx.x, lane = t & 31;
     uint32_t* seg_start = b.seg_start + im.seg_first;
     uint32_t* seg_end   = b.seg_end + im.seg_first;
     if (t == 0) seg_start[0] = 0;
@@ -121,20 +122,10 @@ __global__ void __launch_bounds__(MS_THREADS) k_marker_scan(DevBatch b)
             if (off0 >= term) mask = 0;
             else if (term - off0 < 64) mask &= (1ull << (uint32_t)(term - off0)) - 1ull;
         }
-        uint32_t cnt = __popcll(mask);
-        // block exclusive scan of cnt
-        uint32_t inc = cnt;
-        #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { uint32_t y = __shfl_up_sync(FULL, inc, d); if (lane >= d) inc += y; }
-        if (lane == 31) s_warp[wid] = inc;
-        __syncthreads();
-        uint32_t wbase = 0, total = 0;
-        #pragma unroll
-        for (int w = 0; w < MS_THREADS / 32; w++) { uint32_t y = s_warp[w]; if (w < wid) wbase += y; total += y; }
-        ms_record_rst(b, blockIdx.x, seg_start, seg_end, im.nseg, p, mask, (uint32_t)off0, found + wbase + inc - cnt);
-        found += total;
+        // the scan's leading barrier also orders this pass's reads of s_term before the next pass rewrites it
+        const uint32_t rank = js_block_scan<MS_THREADS>((uint32_t)__popcll(mask), 0u, js_add, found, s_warp);
+        ms_record_rst(b, blockIdx.x, seg_start, seg_end, im.nseg, p, mask, (uint32_t)off0, rank);
         if (term != 0xffffffffu) break;
-        __syncthreads();                    // s_warp / s_term are rewritten by the next pass
     }
     __syncthreads();
     if (t == 0) ms_close(b, blockIdx.x, im, found, (term != 0xffffffffu) ? term : (uint32_t)n);
@@ -219,9 +210,8 @@ __global__ void __launch_bounds__(256) k_marker_scan2(DevBatch b)
                 if (pos0 >= cterm) rst[r] = 0; else if (cterm - pos0 < 16) rst[r] &= (1u << (cterm - pos0)) - 1u;
             }
             const uint32_t cnt = __popc(rst[r]);
-            uint32_t inc = cnt;
-            #pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(FULL, inc, d); if (lane >= d) inc += y; }
+            uint32_t inc;
+            js_warp_scan(cnt, 0u, js_add, inc);              // inc - cnt: the exclusive rank without the scan's extra shuffle
             cntp[r] = total + inc - cnt;
             total += __shfl_sync(FULL, inc, 31);
         }

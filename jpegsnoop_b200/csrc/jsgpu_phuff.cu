@@ -14,6 +14,7 @@
 // Afterwards k_huff_lane<.., VSEG = true> (jsgpu_huff.cu) decodes every slot as a virtual restart interval.
 // Reference semantics matched: CimgDecode::DecodeScanImg's serial MCU walk, ImgDecode.cpp:3164-3630.
 #include "jsgpu_phuff_core.cuh"
+#include "jsgpu_scan.cuh"
 #include <algorithm>
 
 #define FULL 0xffffffffu
@@ -138,8 +139,8 @@ __global__ void __launch_bounds__(PH_THREADS) k_ph_fix_cta(DevBatch b)
 __global__ void __launch_bounds__(256) k_ph_scan(DevBatch b)
 {
     __shared__ uint4 s_w[8];
-    __shared__ uint4 s_carry;
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint4 zero = make_uint4(0, 0, 0, 0);
+    const auto add = [](uint4 a, uint4 c) { return make_uint4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w); };
     for (uint32_t ii = blockIdx.x; ii < b.nimg; ii += gridDim.x) {
         const DevImage& im = b.img[ii];
         if (!im.valid || !im.psync) continue;
@@ -149,32 +150,11 @@ __global__ void __launch_bounds__(256) k_ph_scan(DevBatch b)
             if (!ulen) atomicOr(&b.img_status[ii], 2u);
         }
         const uint4* cnt = b.ph_cnt + im.ph_first; uint4* pre = b.ph_pre + im.ph_first;
-        __syncthreads();
-        if (threadIdx.x == 0) s_carry = make_uint4(0, 0, 0, 0);
-        __syncthreads();
+        uint4 carry = zero;
         for (uint32_t base = 0; base <= im.ph_nslots; base += 256) {
             const uint32_t slot = base + threadIdx.x;
-            const uint4 v = (slot < im.ph_nslots) ? cnt[slot] : make_uint4(0, 0, 0, 0);
-            uint4 inc = v;
-            #pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const uint32_t x = __shfl_up_sync(FULL, inc.x, d), y = __shfl_up_sync(FULL, inc.y, d), z = __shfl_up_sync(FULL, inc.z, d), w = __shfl_up_sync(FULL, inc.w, d);
-                if (lane >= (uint32_t)d) { inc.x += x; inc.y += y; inc.z += z; inc.w += w; }
-            }
-            if (lane == 31) s_w[wid] = inc;
-            __syncthreads();
-            uint4 wb = make_uint4(0, 0, 0, 0), tot = make_uint4(0, 0, 0, 0);
-            #pragma unroll
-            for (int q = 0; q < 8; q++) {
-                const uint4 y = s_w[q];
-                if (q < (int)wid) { wb.x += y.x; wb.y += y.y; wb.z += y.z; wb.w += y.w; }
-                tot.x += y.x; tot.y += y.y; tot.z += y.z; tot.w += y.w;
-            }
-            const uint4 cy = s_carry;
-            if (slot <= im.ph_nslots) pre[slot] = make_uint4(cy.x + wb.x + inc.x - v.x, cy.y + wb.y + inc.y - v.y, cy.z + wb.z + inc.z - v.z, cy.w + wb.w + inc.w - v.w);
-            __syncthreads();
-            if (threadIdx.x == 0) s_carry = make_uint4(cy.x + tot.x, cy.y + tot.y, cy.z + tot.z, cy.w + tot.w);
-            __syncthreads();
+            const uint4 ex = js_block_scan<256>((slot < im.ph_nslots) ? cnt[slot] : zero, zero, add, carry, s_w);
+            if (slot <= im.ph_nslots) pre[slot] = ex;
         }
     }
 }

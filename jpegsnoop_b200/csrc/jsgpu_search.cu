@@ -21,6 +21,7 @@
 // The first-match value search of Img Search Fwd / Rev (jsgpu_find_value), the every-match value search (jsgpu_find_all)
 // and the extract walk's marker search (jsgpu_find_markers), all at the end of the file, share them.
 #include "jsgpu_internal.h"
+#include "jsgpu_scan.cuh"
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -32,71 +33,6 @@
 #define SR_HALO     272                  // bytes staged past the tile: maxlen - 1 (<= 255) and the 8-byte window, rounded to 16
 #define SR_HBITS    16                   // prefix hash width
 #define SR_WORDS    (SR_TILE / 32)       // match-bitmap words per pattern and tile
-
-// ---- scans: every kernel's, over any T of 32-bit words and any associative op (op(a, b): a, then b) with identity id ----
-template <typename T, typename F>
-__device__ __forceinline__ T sr_shfl(T x, F f)             // f (a shuffle) applied to each 32-bit word of x
-{
-    static_assert(sizeof(T) % 4 == 0, "shuffled as 32-bit words");
-    uint32_t w[sizeof(T) / 4];
-    memcpy(w, &x, sizeof(T));
-#pragma unroll
-    for (int i = 0; i < (int)(sizeof(T) / 4); i++) w[i] = f(w[i]);
-    memcpy(&x, w, sizeof(T));
-    return x;
-}
-
-// Over lanes 0 .. W-1 (W a power of two; the whole warp calls): returns the exclusive prefix of v, id in lane 0, and sets
-// `inc` to the inclusive one.
-template <int W = 32, typename T, typename Op>
-__device__ __forceinline__ T warp_scan(T v, T id, Op op, T& inc)
-{
-    const uint32_t lane = threadIdx.x & 31;
-    inc = v;
-#pragma unroll
-    for (int d = 1; d < W; d <<= 1) {
-        const T o = sr_shfl(inc, [d](uint32_t x) { return __shfl_up_sync(0xffffffffu, x, d); });
-        if (lane >= (uint32_t)d) inc = op(o, inc);
-    }
-    const T ex = sr_shfl(inc, [](uint32_t x) { return __shfl_up_sync(0xffffffffu, x, 1); });
-    return lane ? ex : id;
-}
-__device__ __forceinline__ uint32_t sr_add(uint32_t a, uint32_t b) { return a + b; }
-
-// Over a CTA of NT threads, after `carry` (the same in every thread): returns carry op (the values of the threads before
-// this one) and advances `carry` by the whole CTA's.  s_w: NT / 32 + 1 elements of shared memory, free again at the next
-// call.  Up to 8 warps, every thread combines the warp totals itself, which takes no barrier after that of the totals.
-// With more, 32 serial steps in every thread would cost more than a barrier: warp 0 scans the totals for all.
-template <int NT, typename T, typename Op>
-__device__ __forceinline__ T block_scan(T v, T id, Op op, T& carry, T* s_w)
-{
-    constexpr uint32_t NW = NT / 32;
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    T inc, before = carry;
-    const T ex = warp_scan(v, id, op, inc);
-    __syncthreads();                                          // the previous call is done with s_w
-    if (lane == 31) s_w[warp] = inc;
-    __syncthreads();
-    if constexpr (NW <= 8) {
-#pragma unroll
-        for (uint32_t k = 0; k < NW; k++) {
-            const T w = s_w[k];
-            if (k < warp) before = op(before, w);
-            carry = op(carry, w);
-        }
-    } else {
-        if (warp == 0) {                                      // s_w[w] becomes carry op the warps before w, s_w[NW] the new carry
-            const T wex = warp_scan<NW>(lane < NW ? s_w[lane] : id, id, op, inc);
-            __syncwarp();
-            if (lane < NW) s_w[lane] = op(carry, wex);
-            if (lane == NW - 1) s_w[NW] = op(carry, inc);
-        }
-        __syncthreads();
-        before = s_w[warp];
-        carry = s_w[NW];
-    }
-    return op(before, ex);
-}
 
 struct SrParams {
     uint32_t npat, maxlen;
@@ -216,7 +152,7 @@ k_search_tiles(const uint8_t* __restrict__ chunk, uint64_t chunk_pos, uint64_t v
         for (uint32_t k = warp; k < npat; k += SR_THREADS / 32) {
             const uint64_t b0 = ((const uint64_t*)s_match[k])[2 * lane], b1 = ((const uint64_t*)s_match[k])[2 * lane + 1];
             uint32_t inc;
-            const uint32_t pre = warp_scan(sr_then(sr_word_map(b0), sr_word_map(b1)), 2u, sr_then, inc);
+            const uint32_t pre = js_warp_scan(sr_then(sr_word_map(b0), sr_word_map(b1)), 2u, sr_then, inc);
             if (!EMIT) {
                 const uint32_t tot = __shfl_sync(0xffffffffu, inc, 31);
                 uint64_t r0, r1;
@@ -230,7 +166,7 @@ k_search_tiles(const uint8_t* __restrict__ chunk, uint64_t chunk_pos, uint64_t v
                 uint64_t r0, r1;
                 sr_lane_bits(b0, b1, pre, o & 1u, r0, r1);
                 uint32_t n_inc;                                  // j: chunk-local output index of this lane's first position
-                uint32_t j = (o >> 1) + warp_scan((uint32_t)(__popcll(r0) + __popcll(r1)), 0u, sr_add, n_inc);
+                uint32_t j = (o >> 1) + js_warp_scan((uint32_t)(__popcll(r0) + __popcll(r1)), 0u, js_add, n_inc);
                 const uint32_t fp0 = (uint32_t)(chunk_pos + tb) + 128 * lane;
                 for (int h = 0; h < 2; h++) {
                     uint64_t r = h ? r1 : r0;
@@ -274,7 +210,7 @@ k_search_scan(const uint32_t* __restrict__ summ, uint32_t ntiles, uint32_t* __re
             const uint32_t s = summ[(size_t)k * ntiles + t];
             m.c0 = s & 0xFFFu; m.c1 = (s >> 12) & 0xFFFu; m.o0 = (s >> 24) & 1u; m.o1 = (s >> 25) & 1u;
         }
-        const SrMap ex = block_scan<1024>(m, id, sr_compose, all, s_w);
+        const SrMap ex = js_block_scan<1024>(m, id, sr_compose, all, s_w);
         if (t < ntiles) toff[(size_t)k * ntiles + t] = ((r ? ex.c1 : ex.c0) << 1) | (r ? ex.o1 : ex.o0);
     }
     if (tid == 0) {
@@ -687,7 +623,7 @@ k_find_all(const uint8_t* __restrict__ buf, uint32_t npos, FaSets sets, uint32_t
         if (ck[blockIdx.x] == 0 || j >= f.cap) continue;
         for (uint32_t t = t0; t < t1 && j < f.cap; t++) {
             uint32_t m = fa_match16(buf, t * SR_TILE + 16 * tid, f);
-            uint64_t o = block_scan<SR_THREADS>((uint32_t)__popc(m), 0u, sr_add, j, s_w);   // advances j past the tile
+            uint64_t o = js_block_scan<SR_THREADS>((uint32_t)__popc(m), 0u, js_add, j, s_w);   // advances j past the tile
             const uint32_t p = chunk_pos + t * SR_TILE + 16 * tid;
             while (m && o < f.cap) { f.out[o++] = p + (uint32_t)__ffs((int)m) - 1; m &= m - 1; }
         }
@@ -703,7 +639,7 @@ k_find_all_scan(uint32_t* __restrict__ cta, uint32_t ncta, uint32_t* __restrict_
     uint32_t run = *total;
     for (uint32_t b0 = 0; b0 < ncta; b0 += 1024) {
         const uint32_t b = b0 + threadIdx.x;
-        const uint32_t o = block_scan<1024>(b < ncta ? cta[b] : 0u, 0u, sr_add, run, s_w);
+        const uint32_t o = js_block_scan<1024>(b < ncta ? cta[b] : 0u, 0u, js_add, run, s_w);
         if (b < ncta) cta[ncta + b] = o;
     }
     if (threadIdx.x == 0) *total = run;
